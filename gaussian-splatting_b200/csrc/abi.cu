@@ -110,10 +110,21 @@ static int make_cam(const GsbSettings *s, CamArgs &c) {
     return GSB_OK;
 }
 
-static int check_inputs(const GsbSettings *s, const GsbInputs *in) {
+// split: the split SH input of gsb_forward_split_sh / gsb_backward_split_sh (its dc takes the place of in->shs), or NULL
+static int check_inputs(const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split = nullptr) {
     if (in->P < 0) { set_error("inputs: P < 0"); return GSB_ERR_ARGUMENT; }
     if (in->P > 0 && (!in->means3D || !in->opacities)) { set_error("inputs: means3D / opacities missing"); return GSB_ERR_ARGUMENT; }
-    if (in->P > 0 && ((in->shs != nullptr) == (in->colors_precomp != nullptr))) {
+    if (split) {
+        if (in->shs) { set_error("split SH input: in->shs must be NULL (dc and rest carry the coefficients)"); return GSB_ERR_ARGUMENT; }
+        if (split->dc && in->colors_precomp) { set_error("split SH input: dc given together with colors_precomp"); return GSB_ERR_ARGUMENT; }
+        if (split->rest && s->sh_coeffs == 1) { set_error("split SH input: rest given with sh_coeffs == 1"); return GSB_ERR_ARGUMENT; }
+        if (in->P > 0 && split->dc && !split->rest && s->sh_coeffs > 1) {
+            set_error("split SH input: rest missing for sh_coeffs == %d", s->sh_coeffs);
+            return GSB_ERR_ARGUMENT;
+        }
+    }
+    const float *sh = split ? split->dc : in->shs;
+    if (in->P > 0 && ((sh != nullptr) == (in->colors_precomp != nullptr))) {
         set_error("inputs: provide exactly one of shs / colors_precomp");
         return GSB_ERR_ARGUMENT;
     }
@@ -122,7 +133,7 @@ static int check_inputs(const GsbSettings *s, const GsbInputs *in) {
         set_error("inputs: provide exactly one of (scales, rotations) / cov3D_precomp");
         return GSB_ERR_ARGUMENT;
     }
-    if (in->shs && s->sh_coeffs < (s->sh_degree + 1) * (s->sh_degree + 1)) {
+    if (sh && s->sh_coeffs < (s->sh_degree + 1) * (s->sh_degree + 1)) {
         set_error("inputs: shs has %d coefficients, degree %d needs %d", s->sh_coeffs, s->sh_degree,
                   (s->sh_degree + 1) * (s->sh_degree + 1));
         return GSB_ERR_ARGUMENT;
@@ -201,11 +212,12 @@ static int maybe_tile_order(const uint2 *ranges, int V, int num_tiles, uint32_t 
     return launch_tile_order(ranges, V, num_tiles, order, debug, stream);
 }
 
-int32_t gsb_forward(const GsbSettings *s, const GsbInputs *in, float *out_color, int32_t *out_radii,
-                    float *out_invdepth, int64_t capacity_hint, gsb_alloc_fn alloc, void *alloc_ctx, GsbState *st,
-                    void *cuda_stream) {
+// shared body of gsb_forward (split == NULL) and gsb_forward_split_sh
+static int forward_impl(const char *fn, const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, float *out_color,
+                        int32_t *out_radii, float *out_invdepth, int64_t capacity_hint, gsb_alloc_fn alloc, void *alloc_ctx,
+                        GsbState *st, void *cuda_stream) {
     if (!s || !in || !out_color || (!out_radii && in->P > 0) || !out_invdepth || !alloc || !st) {
-        set_error("gsb_forward: NULL argument");
+        set_error("%s: NULL argument", fn);
         return GSB_ERR_ARGUMENT;
     }
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
@@ -213,7 +225,7 @@ int32_t gsb_forward(const GsbSettings *s, const GsbInputs *in, float *out_color,
     CamArgs cam;
     int rc = make_cam(s, cam);
     if (rc) return rc;
-    rc = check_inputs(s, in);
+    rc = check_inputs(s, in, split);
     if (rc) return rc;
     const int P = in->P;
     const int num_tiles = cam.gx * cam.gy;
@@ -299,11 +311,12 @@ int32_t gsb_forward(const GsbSettings *s, const GsbInputs *in, float *out_color,
     int64_t D = 0;
     if (P > 0) {
         PreFwdArgs pa;
-        pa.P = P; pa.means = in->means3D; pa.shs = in->shs; pa.colors = in->colors_precomp; pa.opac = in->opacities;
+        pa.P = P; pa.means = in->means3D; pa.shs = split ? split->dc : in->shs; pa.colors = in->colors_precomp; pa.opac = in->opacities;
         pa.scales = in->scales; pa.rots = in->rotations; pa.cov_pre = in->cov3D_precomp;
+        pa.rest = split ? split->rest : nullptr;
         pa.splat = splat; pa.depth_key = key; pa.depth_idx = idx; pa.tiles = tiles; pa.rect = rect; pa.radii = out_radii;
         pa.cull = opt_cull;
-        rc = launch_preprocess_fwd(cam, pa, debug, stream);
+        rc = launch_preprocess_fwd(cam, pa, split != nullptr, debug, stream);
         if (rc) return rc;
         // gaussians by depth (culled ones carry key 0xffffffff and sort to the end)
         rc = sort_pairs(key, idx, key_alt, idx_alt, P, nullptr, 0, 32, sortscr, debug, stream);
@@ -342,12 +355,27 @@ int32_t gsb_forward(const GsbSettings *s, const GsbInputs *in, float *out_color,
     return GSB_OK;
 }
 
-int32_t gsb_backward(const GsbSettings *s, const GsbInputs *in, const GsbState *st, const float *out_color,
-                     const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
-                     const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx,
-                     void *cuda_stream) {
+int32_t gsb_forward(const GsbSettings *s, const GsbInputs *in, float *out_color, int32_t *out_radii,
+                    float *out_invdepth, int64_t capacity_hint, gsb_alloc_fn alloc, void *alloc_ctx, GsbState *st,
+                    void *cuda_stream) {
+    return forward_impl("gsb_forward", s, in, nullptr, out_color, out_radii, out_invdepth, capacity_hint, alloc, alloc_ctx, st,
+                        cuda_stream);
+}
+
+int32_t gsb_forward_split_sh(const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, float *out_color,
+                             int32_t *out_radii, float *out_invdepth, int64_t capacity_hint, gsb_alloc_fn alloc,
+                             void *alloc_ctx, GsbState *st, void *cuda_stream) {
+    if (!split) { set_error("gsb_forward_split_sh: NULL argument"); return GSB_ERR_ARGUMENT; }
+    return forward_impl("gsb_forward_split_sh", s, in, split, out_color, out_radii, out_invdepth, capacity_hint, alloc, alloc_ctx, st,
+                        cuda_stream);
+}
+
+// shared body of gsb_backward (split == NULL) and gsb_backward_split_sh
+static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
+                         const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
+                         const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {
     if (!s || !in || !st || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc) {
-        set_error("gsb_backward: NULL argument");
+        set_error("%s: NULL argument", fn);
         return GSB_ERR_ARGUMENT;
     }
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
@@ -355,11 +383,15 @@ int32_t gsb_backward(const GsbSettings *s, const GsbInputs *in, const GsbState *
     CamArgs cam;
     int rc = make_cam(s, cam);
     if (rc) return rc;
-    rc = check_inputs(s, in);
+    rc = check_inputs(s, in, split);
     if (rc) return rc;
+    if (split && grads->dL_dshs) {
+        set_error("%s: grads->dL_dshs must be NULL (dL_ddc / dL_drest receive the SH gradient)", fn);
+        return GSB_ERR_ARGUMENT;
+    }
     const int P = in->P;
     if (P != st->P || st->num_tiles != cam.gx * cam.gy || !st->splat || !st->ranges || !st->final_T) {
-        set_error("gsb_backward: state does not match the inputs (P %d vs %d)", P, st->P);
+        set_error("%s: state does not match the inputs (P %d vs %d)", fn, P, st->P);
         return GSB_ERR_ARGUMENT;
     }
     if (P == 0) return GSB_OK;
@@ -381,11 +413,31 @@ int32_t gsb_backward(const GsbSettings *s, const GsbInputs *in, const GsbState *
         if (rc) return rc;
     }
     PreBwdArgs pa;
-    pa.P = P; pa.means = in->means3D; pa.shs = in->shs; pa.opac = in->opacities; pa.scales = in->scales; pa.rots = in->rotations;
-    pa.cov_pre = in->cov3D_precomp; pa.splat = splat; pa.dacc = dacc; pa.g = *grads;
+    pa.P = P; pa.means = in->means3D; pa.shs = split ? split->dc : in->shs; pa.opac = in->opacities; pa.scales = in->scales;
+    pa.rots = in->rotations; pa.cov_pre = in->cov3D_precomp; pa.splat = splat; pa.dacc = dacc; pa.g = *grads;
+    pa.rest = split ? split->rest : nullptr;
+    pa.dL_drest = split ? split->dL_drest : nullptr;
+    if (split) pa.g.dL_dshs = split->dL_ddc;
     pa.p_begin = 0; pa.p_end = P;
     pa.peer.world = 0;
-    return launch_preprocess_bwd(cam, pa, accumulate != 0, debug, stream);
+    return launch_preprocess_bwd(cam, pa, split != nullptr, accumulate != 0, debug, stream);
+}
+
+int32_t gsb_backward(const GsbSettings *s, const GsbInputs *in, const GsbState *st, const float *out_color,
+                     const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
+                     const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx,
+                     void *cuda_stream) {
+    return backward_impl("gsb_backward", s, in, nullptr, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate,
+                         alloc, alloc_ctx, cuda_stream);
+}
+
+int32_t gsb_backward_split_sh(const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
+                              const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                              const float *dL_dinvdepth, const GsbGrads *grads, int32_t accumulate,
+                              gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {
+    if (!split) { set_error("gsb_backward_split_sh: NULL argument"); return GSB_ERR_ARGUMENT; }
+    return backward_impl("gsb_backward_split_sh", s, in, split, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads,
+                         accumulate, alloc, alloc_ctx, cuda_stream);
 }
 
 static int check_batch(int32_t V, const GsbSettings *s, const GsbInputs *in, CamArgsBatch &cb) {
@@ -465,7 +517,7 @@ static int forward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs *
 
     PreFwdArgs pa;
     pa.P = P; pa.means = in->means3D; pa.shs = in->shs; pa.colors = nullptr; pa.opac = in->opacities;
-    pa.scales = in->scales; pa.rots = in->rotations; pa.cov_pre = nullptr;
+    pa.scales = in->scales; pa.rots = in->rotations; pa.cov_pre = nullptr; pa.rest = nullptr;
     pa.splat = splat; pa.depth_key = key; pa.depth_idx = idx; pa.tiles = tiles; pa.rect = rect; pa.radii = out_radii;
     pa.cull = opt_cull;
     PreFwdBatchStrides ps;
@@ -647,6 +699,7 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
     PreBwdArgs pa;
     pa.P = P; pa.means = in->means3D; pa.shs = in->shs; pa.opac = in->opacities; pa.scales = in->scales; pa.rots = in->rotations;
     pa.cov_pre = nullptr; pa.splat = static_cast<const float4 *>(states[0].splat); pa.dacc = dacc; pa.g = *grads;
+    pa.rest = nullptr; pa.dL_drest = nullptr;
     pa.peer.world = 0;
     if (peers) {
         if (peers->world < 1 || peers->world > GSB_MAX_PEERS || peers->rank < 0 || peers->rank >= peers->world ||
@@ -815,6 +868,23 @@ int32_t gsb_adam_step(const GsbAdamArgs *a, void *cuda_stream) {
     if ((a->skip_groups & 0x3f) == 0x3f) return GSB_OK;
     return launch_adam_step(a->P, a->sh_coeffs, a->params, a->grads, a->exp_avg, a->exp_avg_sq, a->act, a->visible, a->step_size,
                             a->beta1, a->beta2, a->eps, a->bias2_sqrt, (uint32_t)a->skip_groups, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int32_t gsb_sparse_adam_step(const GsbSparseAdamGroup *groups, int32_t n_groups, const uint8_t *visible, int64_t N, float beta1,
+                             float beta2, void *cuda_stream) {
+    if (!groups || n_groups < 1 || n_groups > GSB_MAX_SPARSE_GROUPS || N < 0 || (N > 0 && !visible)) {
+        set_error("gsb_sparse_adam_step: bad argument (n_groups %d outside 1..%d, N %lld)", n_groups, GSB_MAX_SPARSE_GROUPS, (long long)N);
+        return GSB_ERR_ARGUMENT;
+    }
+    for (int k = 0; k < n_groups; ++k) {
+        const GsbSparseAdamGroup &g = groups[k];
+        if (g.width <= 0 || N * (int64_t)g.width >= ((int64_t)1 << 31) ||
+            (N > 0 && (!g.param || !g.grad || !g.exp_avg || !g.exp_avg_sq))) {
+            set_error("gsb_sparse_adam_step: group %d: width %d must be positive, N * width below 2^31, pointers non-NULL", k, g.width);
+            return GSB_ERR_ARGUMENT;
+        }
+    }
+    return launch_sparse_adam_step(groups, n_groups, visible, N, beta1, beta2, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int32_t gsb_activate(int64_t P, int32_t sh_coeffs, const float *params, float *act, void *cuda_stream) {

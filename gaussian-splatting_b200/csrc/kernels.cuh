@@ -19,9 +19,13 @@ struct CamArgsBatch {
 struct PreFwdBatchStrides { size_t splat /* float4 */, per_gauss /* u32 / uint2 arrays */, radii; };
 struct PreBwdBatchStrides { size_t splat /* float4 */, dacc /* float */, means2D /* float */; };
 
+// Split SH input (gsb_forward_split_sh / gsb_backward_split_sh, single-view kernels only): `shs` points at the DC rows
+// [P,1,3] and `rest` at the remaining coefficients [P,M-1,3] (NULL when M == 1); the kernels assemble the joint row in
+// shared memory.  Every other launch leaves `rest` (and `dL_drest`) NULL.
 struct PreFwdArgs {
     int P;
     const float *means, *shs, *colors, *opac, *scales, *rots, *cov_pre;
+    const float *rest;
     float4 *splat;        // [P*3]
     uint32_t *depth_key;  // [P] float bits of view depth, 0xffffffff when culled
     uint32_t *depth_idx;  // [P] identity, sorted along with the keys
@@ -48,6 +52,8 @@ struct PreBwdArgs {
     int p_begin, p_end;   // gaussian range of this launch (chunked backward: the caller reduces finished chunks meanwhile)
     GsbGrads g;
     PeerTable peer;       // world > 0: outputs are ADDED into the owners' buffers (view-batch kernel, TMA rows only)
+    const float *rest;    // split SH input: shs = DC rows, g.dL_dshs = their gradient, rest / dL_drest the other coefficients
+    float *dL_drest;
 };
 
 struct BinArgs {
@@ -94,8 +100,9 @@ struct RenderBwdArgs {
     float *dacc;
 };
 
-int launch_preprocess_fwd(const CamArgs &ca, const PreFwdArgs &a, bool debug, cudaStream_t stream);
-int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool accumulate, bool debug, cudaStream_t stream);
+// split: a.shs / a.rest are the split SH input (see PreFwdArgs)
+int launch_preprocess_fwd(const CamArgs &ca, const PreFwdArgs &a, bool split, bool debug, cudaStream_t stream);
+int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool split, bool accumulate, bool debug, cudaStream_t stream);
 int launch_preprocess_fwd_batch(const CamArgsBatch &cb, const PreFwdArgs &a, const PreFwdBatchStrides &st, bool debug, cudaStream_t stream);
 int launch_preprocess_bwd_batch(const CamArgsBatch &cb, const PreBwdArgs &a, const PreBwdBatchStrides &st, bool accumulate, bool debug,
                                 cudaStream_t stream);
@@ -123,6 +130,9 @@ int launch_adam_step(int64_t P, int sh_coeffs, float *params, const float *grads
                      const uint8_t *visible, const float step_size[6], float beta1, float beta2, float eps, const float bias2_sqrt[6],
                      uint32_t skip_groups, cudaStream_t stream);
 int launch_activate(int64_t P, int sh_coeffs, const float *params, float *act, cudaStream_t stream);
+// SparseGaussianAdam: up to GSB_MAX_SPARSE_GROUPS [N, width] groups, rows with visible[i] == 0 untouched (optim.cu)
+int launch_sparse_adam_step(const GsbSparseAdamGroup *groups, int n_groups, const uint8_t *visible, int64_t N, float beta1, float beta2,
+                            cudaStream_t stream);
 size_t densify_scratch_bytes(int64_t P, int n_children);
 // exclusive scan of n uint32 (in == out allowed); partials: scan_u32_partials(n) words; *total receives the sum
 size_t scan_u32_partials(int64_t n);

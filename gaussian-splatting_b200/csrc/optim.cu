@@ -142,6 +142,62 @@ int launch_adam_step(int64_t P, int sh_coeffs, float *params, const float *grads
     return GSB_OK;
 }
 
+// ---- SparseGaussianAdam (train.py --optimizer_type sparse_adam): separate [N, width] tensors per group, one launch ----------
+// The blocks of all groups form one grid, group after group (block0[k] = first block of group k).  A visible row costs
+// 4 loads + 3 stores of 4 bytes per float; an invisible row costs its mask byte only.
+struct SparseAdamK {
+    GsbSparseAdamGroup grp[GSB_MAX_SPARSE_GROUPS];
+    uint32_t block0[GSB_MAX_SPARSE_GROUPS];
+    int n_groups;
+    uint32_t N;
+    const uint8_t *vis;
+    float b1, b2;
+};
+
+__global__ void __launch_bounds__(AD_THREADS)
+sparse_adam_kernel(const SparseAdamK a) {
+    // the block's group, selected with static indices only (a dynamic index into the kernel parameters would copy them to
+    // local memory)
+    GsbSparseAdamGroup G = a.grp[0];
+    uint32_t b0 = 0;
+#pragma unroll
+    for (int k = 1; k < GSB_MAX_SPARSE_GROUPS; ++k)
+        if (k < a.n_groups && blockIdx.x >= a.block0[k]) { G = a.grp[k]; b0 = a.block0[k]; }
+    const AdamCoef c{1.0f - a.b1, a.b2, 1.0f - a.b2, G.eps};
+    const uint32_t w = (uint32_t)G.width, E = a.N * w;
+    const uint32_t base = (blockIdx.x - b0) * (AD_THREADS * AD_UNROLL) + threadIdx.x;
+    float p[AD_UNROLL], g[AD_UNROLL], m[AD_UNROLL], v[AD_UNROLL];
+    bool on[AD_UNROLL];
+#pragma unroll
+    for (int u = 0; u < AD_UNROLL; ++u) {
+        const uint32_t e = base + u * AD_THREADS;
+        on[u] = e < E && a.vis[e / w] != 0;
+        if (on[u]) { p[u] = G.param[e]; g[u] = G.grad[e]; m[u] = G.exp_avg[e]; v[u] = G.exp_avg_sq[e]; }
+    }
+#pragma unroll
+    for (int u = 0; u < AD_UNROLL; ++u) {
+        if (!on[u]) continue;
+        const uint32_t e = base + u * AD_THREADS;
+        adam_update(p[u], m[u], v[u], g[u], G.lr, 1.0f, c);     // step_size = lr, bias2_sqrt = 1: no bias correction
+        G.param[e] = p[u]; G.exp_avg[e] = m[u]; G.exp_avg_sq[e] = v[u];
+    }
+}
+
+int launch_sparse_adam_step(const GsbSparseAdamGroup *groups, int n_groups, const uint8_t *visible, int64_t N, float beta1, float beta2,
+                            cudaStream_t stream) {
+    if (N == 0) return GSB_OK;
+    SparseAdamK a{};
+    uint32_t blocks = 0;
+    for (int k = 0; k < n_groups; ++k) {
+        a.grp[k] = groups[k];
+        a.block0[k] = blocks;
+        blocks += (uint32_t)ceil_div(N * groups[k].width, AD_THREADS * AD_UNROLL);
+    }
+    a.n_groups = n_groups; a.N = (uint32_t)N; a.vis = visible; a.b1 = beta1; a.b2 = beta2;
+    GSB_LAUNCH("sparse_adam", false, stream, sparse_adam_kernel, blocks, AD_THREADS, 0, a);
+    return GSB_OK;
+}
+
 int launch_activate(int64_t P, int sh_coeffs, const float *params, float *act, cudaStream_t stream) {
     if (P == 0) return GSB_OK;
     const size_t e_op = (size_t)(3 + 3 * sh_coeffs) * P;

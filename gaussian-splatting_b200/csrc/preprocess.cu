@@ -238,6 +238,79 @@ __device__ __forceinline__ void stage_rows_out(float *__restrict__ g, const floa
     }
 }
 
+// ---- third staging source: split SH input (DC rows [P,1,3] and rest rows [P,M-1,3] in two tensors) ----------------------------
+// Each source's span for the block ([nrows, n] floats) is contiguous in global memory and is moved with word accesses,
+// consecutive threads on consecutive words (coalesced), into / out of columns [col0, col0 + ncols) of the joint rows that
+// stage_rows_in lays out in shared memory (odd word stride).  Everything after staging is the joint path's code.
+__device__ __forceinline__ void stage_span_in(const float *__restrict__ g, float *s, const int row0, const int nrows, const int n,
+                                              const int ncols, const int stride, const int col0) {
+    if (ncols <= 0) return;
+    const float *gb = g + (size_t)row0 * n;
+    const int total = nrows * ncols;
+    const float inv = 1.0f / (float)ncols;
+    for (int base = 0; base < total; base += 4 * PRE_THREADS) {
+        float v[4];
+        int si[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int idx = base + u * PRE_THREADS + threadIdx.x;
+            si[u] = -1;
+            if (idx < total) {
+                const int r = (int)(((float)idx + 0.5f) * inv), c = idx - r * ncols;
+                si[u] = r * stride + col0 + c;
+                v[u] = __ldg(gb + (size_t)r * n + c);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+            if (si[u] >= 0) s[si[u]] = v[u];
+    }
+}
+
+template <bool ACC>
+__device__ __forceinline__ void stage_span_out(float *__restrict__ g, const float *s, const int row0, const int nrows, const int n,
+                                               const int stride, const int col0) {
+    if (!g || n <= 0) return;
+    float *gb = g + (size_t)row0 * n;
+    const int total = nrows * n;
+    const float inv = 1.0f / (float)n;
+    for (int base = 0; base < total; base += 4 * PRE_THREADS) {
+        float v[4];
+        int gi[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int idx = base + u * PRE_THREADS + threadIdx.x;
+            gi[u] = -1;
+            if (idx < total) {
+                const int r = (int)(((float)idx + 0.5f) * inv), c = idx - r * n;
+                gi[u] = idx;
+                v[u] = s[r * stride + col0 + c];
+                if (ACC) v[u] += gb[idx];
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+            if (gi[u] >= 0) gb[gi[u]] = v[u];
+    }
+}
+
+// first `ncols` floats of the block's joint rows (row length n = 3M) from the two split tensors (rest may be NULL: M == 1)
+__device__ __forceinline__ void stage_split_rows_in(const float *__restrict__ dc, const float *__restrict__ rest, float *s, const int row0,
+                                                    const int nrows, const int n, const int ncols) {
+    const int stride = sh_row_stride(n);
+    stage_span_in(dc, s, row0, nrows, 3, min(ncols, 3), stride, 0);
+    if (rest) stage_span_in(rest, s, row0, nrows, n - 3, ncols - 3, stride, 3);
+}
+
+// full joint (gradient) rows back to the two split tensors; a NULL destination is skipped
+template <bool ACC>
+__device__ __forceinline__ void stage_split_rows_out(float *__restrict__ ddc, float *__restrict__ drest, const float *s, const int row0,
+                                                     const int nrows, const int n) {
+    const int stride = sh_row_stride(n);
+    stage_span_out<ACC>(ddc, s, row0, nrows, 3, stride, 0);
+    stage_span_out<ACC>(drest, s, row0, nrows, n - 3, stride, 3);
+}
+
 // one gaussian, one view: everything of K1 after the SH row has been staged
 template <bool VEC>
 __device__ __forceinline__ void preprocess_fwd_body(const CamParams &cam, const PreFwdArgs &a, const int i, const float *sh_row) {
@@ -334,7 +407,8 @@ __device__ __forceinline__ void preprocess_fwd_body(const CamParams &cam, const 
     a.radii[i] = radius_out;
 }
 
-template <bool TMA>
+// SPLIT: split SH input (a.shs = DC rows, a.rest = the other coefficients), staged into the scalar row layout (TMA false)
+template <bool TMA, bool SPLIT = false>
 __global__ void __launch_bounds__(PRE_THREADS)
 preprocess_fwd_kernel(const CamArgs ca, const PreFwdArgs a) {
     __shared__ CamParams cam;
@@ -346,7 +420,8 @@ preprocess_fwd_kernel(const CamArgs ca, const PreFwdArgs a) {
     const int nrows = min(PRE_THREADS, a.P - row0);
     const int shn = 3 * ca.sh_coeffs;
     if (a.shs) {
-        if (TMA) tma_rows_in(a.shs, sh_rows, &bar, row0, nrows, shn);
+        if (SPLIT) stage_split_rows_in(a.shs, a.rest, sh_rows, row0, nrows, shn, 3 * (ca.sh_degree + 1) * (ca.sh_degree + 1));
+        else if (TMA) tma_rows_in(a.shs, sh_rows, &bar, row0, nrows, shn);
         else stage_rows_in(a.shs, sh_rows, row0, nrows, shn, 3 * (ca.sh_degree + 1) * (ca.sh_degree + 1));
     }
     __syncthreads();
@@ -632,8 +707,8 @@ __device__ __forceinline__ T *shift_ptr(T *p, const long long bytes) {
     return reinterpret_cast<T *>(reinterpret_cast<char *>(p) + bytes);
 }
 
-// K8, one view.
-template <bool ACC, bool TMA>
+// K8, one view.  SPLIT: split SH input and gradient (a.shs / a.g.dL_dshs = DC rows, a.rest / a.dL_drest = the rest; TMA false).
+template <bool ACC, bool TMA, bool SPLIT = false>
 __global__ void __launch_bounds__(PRE_THREADS)
 preprocess_bwd_kernel(const CamArgs ca, const PreBwdArgs a) {
     __shared__ CamParams cam;
@@ -646,7 +721,8 @@ preprocess_bwd_kernel(const CamArgs ca, const PreBwdArgs a) {
     const int shn = 3 * ca.sh_coeffs;
     const int nb = (ca.sh_degree + 1) * (ca.sh_degree + 1);
     if (a.shs) {
-        if (TMA) tma_rows_in(a.shs, sh_rows, &bar, row0, nrows, shn);
+        if (SPLIT) stage_split_rows_in(a.shs, a.rest, sh_rows, row0, nrows, shn, 3 * nb);
+        else if (TMA) tma_rows_in(a.shs, sh_rows, &bar, row0, nrows, shn);
         else stage_rows_in(a.shs, sh_rows, row0, nrows, shn, 3 * nb);
     }
     __syncthreads();
@@ -658,13 +734,14 @@ preprocess_bwd_kernel(const CamArgs ca, const PreBwdArgs a) {
     if (live) preprocess_bwd_view<TMA>(cam, a, i, sh_row, __float_as_uint(a.splat[(size_t)i * SPLAT_F4 + 2].w), g);
 
     // SH gradient rows go out through shared memory (coalesced / one bulk store); each thread rewrites only its own row
-    if (a.g.dL_dshs && a.shs) {
+    if ((a.g.dL_dshs || (SPLIT && a.dL_drest)) && a.shs) {
         if (live) sh_grad_row<TMA, false>(sh_row, g.bas, g.d_rgb_sh, nb, M);
         if (TMA) {
             tma_row_out<ACC>(a.g.dL_dshs, sh_row, i, shn, live);
         } else {
             __syncthreads();
-            stage_rows_out<ACC>(a.g.dL_dshs, sh_rows, row0, nrows, shn);
+            if (SPLIT) stage_split_rows_out<ACC>(a.g.dL_dshs, a.dL_drest, sh_rows, row0, nrows, shn);
+            else stage_rows_out<ACC>(a.g.dL_dshs, sh_rows, row0, nrows, shn);
         }
     }
     if (!live) return;
@@ -813,24 +890,29 @@ static size_t sh_smem_bytes(bool tma, int sh_coeffs, int rows_per_thread) {
         GSB_LAUNCH(name, debug, stream, kernel, grid, PRE_THREADS, smem, __VA_ARGS__);                                      \
     } while (0)
 
-int launch_preprocess_fwd(const CamArgs &ca, const PreFwdArgs &a, bool debug, cudaStream_t stream) {
+// split: split SH input (12-byte DC rows next to the rest rows: no TMA row copies, the scalar row layout is staged from both)
+int launch_preprocess_fwd(const CamArgs &ca, const PreFwdArgs &a, bool split, bool debug, cudaStream_t stream) {
     if (a.P <= 0) return GSB_OK;
     const char *name = "preprocess_fwd";
-    const bool tma = use_tma_rows(a.shs, nullptr, ca.sh_coeffs);
+    const bool tma = !split && use_tma_rows(a.shs, nullptr, ca.sh_coeffs);
     const size_t smem = a.shs ? sh_smem_bytes(tma, ca.sh_coeffs, 1) : 0;
     const int grid = (int)ceil_div(a.P, PRE_THREADS);
-    if (tma) GSB_PRE_LAUNCH(preprocess_fwd_kernel<true>, grid, smem, ca, a);
+    if (split) GSB_PRE_LAUNCH((preprocess_fwd_kernel<false, true>), grid, smem, ca, a);
+    else if (tma) GSB_PRE_LAUNCH(preprocess_fwd_kernel<true>, grid, smem, ca, a);
     else GSB_PRE_LAUNCH(preprocess_fwd_kernel<false>, grid, smem, ca, a);
     return GSB_OK;
 }
 
-int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool accumulate, bool debug, cudaStream_t stream) {
+int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool split, bool accumulate, bool debug, cudaStream_t stream) {
     if (a.P <= 0 || a.p_end <= a.p_begin) return GSB_OK;
     const char *name = "preprocess_bwd";
     const int grid = (int)ceil_div(a.p_end - a.p_begin, PRE_THREADS);
-    const bool tma = use_tma_rows(a.shs, a.g.dL_dshs, ca.sh_coeffs);
+    const bool tma = !split && use_tma_rows(a.shs, a.g.dL_dshs, ca.sh_coeffs);
     const size_t smem = a.shs ? sh_smem_bytes(tma, ca.sh_coeffs, 1) : 0;
-    if (accumulate) {
+    if (split) {
+        if (accumulate) GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, false, true>), grid, smem, ca, a);
+        else GSB_PRE_LAUNCH((preprocess_bwd_kernel<false, false, true>), grid, smem, ca, a);
+    } else if (accumulate) {
         if (tma) GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, true>), grid, smem, ca, a);
         else GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, false>), grid, smem, ca, a);
     } else {

@@ -2,8 +2,15 @@
 
 Mirrors the surface the reference imports at /root/reference/gaussian_renderer/__init__.py:14
 (``GaussianRasterizationSettings``, ``GaussianRasterizer``) and calls at :36-52 / :91-110, plus the
-``rasterize_gaussians`` autograd.Function named in BASELINE.json north_star.  ``SparseGaussianAdam``
-is deliberately NOT exported: its presence would flip ``separate_sh`` in train.py:38,111.
+``rasterize_gaussians`` autograd.Function named in BASELINE.json north_star.  ``GaussianRasterizer.forward`` also
+takes the split SH input of the accel branch (``dc=features_dc, shs=features_rest``).
+
+``SparseGaussianAdam`` (sparse_adam.py, train.py --optimizer_type sparse_adam) is bound at package top level only
+when ``GSB_SPARSE_ADAM=1`` is set at import.  Its presence makes the reference scripts pass ``separate_sh=True``
+(train.py:38,111, render.py:24), and the reference render() then binds ``dc`` only on its SH branch
+(gaussian_renderer/__init__.py:83): ``--convert_SHs_python`` and ``override_color`` raise UnboundLocalError there, as
+they do with the accel rasterizer.  Without the variable those flags keep working and the optimizer stays importable
+as ``diff_gaussian_rasterization.sparse_adam.SparseGaussianAdam``.
 
 There is no CPU path and no fallback: importing this package without the built library raises.
 Host code is plumbing only -- tensors in, raw device pointers across the C ABI (include/gs_b200.h).
@@ -76,6 +83,18 @@ class _DensifyArgs(Structure):       # GsbDensifyArgs
                 ("size_limit", c_float), ("min_opacity", c_float), ("world_limit", c_float), ("scratch", c_void_p)]
 
 
+class _SplitSH(Structure):           # GsbSplitSH
+    _fields_ = [("dc", c_void_p), ("rest", c_void_p), ("dL_ddc", c_void_p), ("dL_drest", c_void_p)]
+
+
+class _SparseAdamGroup(Structure):   # GsbSparseAdamGroup
+    _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p), ("width", c_int32),
+                ("lr", c_float), ("eps", c_float)]
+
+
+MAX_SPARSE_GROUPS = 8               # GSB_MAX_SPARSE_GROUPS: groups per gsb_sparse_adam_step launch
+
+
 def _load(path: Optional[str] = None):
     """Loads libgs_b200.so (or another build of the same C ABI at ``path``) and declares the prototypes."""
     _LIB_PATH = path or globals()["_LIB_PATH"]
@@ -90,6 +109,14 @@ def _load(path: Optional[str] = None):
     lib.gsb_backward.restype = c_int32
     lib.gsb_backward.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_State), c_void_p, c_void_p, c_void_p,
                                  c_void_p, POINTER(_Grads), c_int32, _ALLOC_FN, c_void_p, c_void_p]
+    lib.gsb_forward_split_sh.restype = c_int32
+    lib.gsb_forward_split_sh.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), c_void_p, c_void_p, c_void_p,
+                                         c_int64, _ALLOC_FN, c_void_p, POINTER(_State), c_void_p]
+    lib.gsb_backward_split_sh.restype = c_int32
+    lib.gsb_backward_split_sh.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), POINTER(_State), c_void_p,
+                                          c_void_p, c_void_p, c_void_p, POINTER(_Grads), c_int32, _ALLOC_FN, c_void_p, c_void_p]
+    lib.gsb_sparse_adam_step.restype = c_int32
+    lib.gsb_sparse_adam_step.argtypes = [POINTER(_SparseAdamGroup), c_int32, c_void_p, c_int64, c_float, c_float, c_void_p]
     lib.gsb_forward_batch.restype = c_int32
     lib.gsb_forward_batch.argtypes = [c_int32, POINTER(_Settings), POINTER(_Inputs), c_void_p, c_void_p, c_void_p, c_int64,
                                       _ALLOC_FN, c_void_p, POINTER(_State), c_void_p]
@@ -311,6 +338,26 @@ def adam_step(params, grads, exp_avg, exp_avg_sq, act, P: int, sh_coeffs: int, s
         _check(_C.gsb_adam_step(byref(a), stream))
 
 
+def sparse_adam_step(groups, visible: torch.Tensor, N: int, beta1: float = 0.9, beta2: float = 0.999) -> None:
+    """gsb_sparse_adam_step: ONE launch over 1..MAX_SPARSE_GROUPS groups ``(param, grad, exp_avg, exp_avg_sq, lr, eps)``, each
+    tensor [N, ...] float32 contiguous on the device of ``visible`` ([N] bool or uint8, contiguous).  Rows with visible == 0
+    are left untouched.  No host synchronisation; the caller validates shapes (SparseGaussianAdam.step)."""
+    if not 1 <= len(groups) <= MAX_SPARSE_GROUPS:
+        raise ValueError(f"sparse_adam_step: {len(groups)} groups, 1..{MAX_SPARSE_GROUPS} per launch")
+    N = int(N)
+    if N == 0:
+        return
+    vis = visible.contiguous()
+    vis = vis.view(torch.uint8) if vis.dtype == torch.bool else vis.to(torch.uint8)
+    arr = (_SparseAdamGroup * len(groups))()
+    for k, (p, g, m, v, lr, eps) in enumerate(groups):
+        arr[k].param, arr[k].grad, arr[k].exp_avg, arr[k].exp_avg_sq = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
+        arr[k].width, arr[k].lr, arr[k].eps = p.numel() // N, float(lr), float(eps)
+    stream = _stream_of(vis)
+    with _device_ctx(vis.device):
+        _check(_C.gsb_sparse_adam_step(arr, len(groups), vis.data_ptr(), N, float(beta1), float(beta2), stream))
+
+
 def activate(params: torch.Tensor, act: torch.Tensor, P: int, sh_coeffs: int) -> None:
     stream = _stream_of(params)
     with _device_ctx(params.device):
@@ -474,17 +521,28 @@ _capacity_hints = {}
 speculative_binning = True
 
 
-def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs):
-    """Returns (color, radii, invdepth, ctx_pack).  All tensor arguments already float32-contiguous or None."""
+def _split_sh(dc, rest, grads: Optional[dict] = None) -> _SplitSH:
+    sp = _SplitSH()
+    sp.dc, sp.rest = _ptr(dc), _ptr(rest)
+    if grads is not None:
+        sp.dL_ddc, sp.dL_drest = _ptr(grads.get("dc")), _ptr(grads.get("shs"))
+    return sp
+
+
+def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, dc=None):
+    """Returns (color, radii, invdepth, ctx_pack).  All tensor arguments already float32-contiguous or None.
+    ``dc`` (split SH input, gsb_forward_split_sh): the DC rows [P,1,3]; ``sh`` is then the rest [P,M-1,3] or None."""
     _require_cuda(means3D)
     dev = means3D.device
     P = int(means3D.shape[0])
     H, W = int(rs.image_height), int(rs.image_width)
     M = int(sh.shape[1]) if sh is not None else 0
+    if dc is not None:
+        M += 1
     with _device_ctx(dev):
         keep = []
         cs = _c_settings(rs, M, keep)
-        ci = _c_inputs(P, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+        ci = _c_inputs(P, means3D, sh if dc is None else None, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
         color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((P,), dtype=torch.int32, device=dev)
         invdepth = torch.empty((1, H, W), dtype=torch.float32, device=dev)
@@ -493,8 +551,13 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
         st = _State()
         hkey = (P, H, W, dev.index)
         hint = _capacity_hints.get(hkey, 0) if speculative_binning else 0
-        rc = _C.gsb_forward(byref(cs), byref(ci), color.data_ptr(), radii.data_ptr(), invdepth.data_ptr(), hint,
-                            arena.cb, None, byref(st), stream)
+        if dc is None:
+            rc = _C.gsb_forward(byref(cs), byref(ci), color.data_ptr(), radii.data_ptr(), invdepth.data_ptr(), hint,
+                                arena.cb, None, byref(st), stream)
+        else:
+            sp = _split_sh(dc, sh)
+            rc = _C.gsb_forward_split_sh(byref(cs), byref(ci), byref(sp), color.data_ptr(), radii.data_ptr(), invdepth.data_ptr(),
+                                         hint, arena.cb, None, byref(st), stream)
         _check(rc, arena)
         # next estimate: this count + 25 %, rounded up to 1 Mi instances and never shrinking, so that buffer sizes
         # settle after the first few views instead of following every view's own count
@@ -506,9 +569,10 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
 
 def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                    out_color, out_invdepth, grad_color, grad_invdepth, grads: dict, accumulate: bool,
-                   accumulate_means2D: Optional[bool] = None):
+                   accumulate_means2D: Optional[bool] = None, dc=None):
     """grads: tensors to fill (accumulate=False) or add into (accumulate=True).  The C ABI has one accumulate
-    switch; a per-view means2D buffer (accumulate_means2D=False while the rest accumulates) is zeroed here."""
+    switch; a per-view means2D buffer (accumulate_means2D=False while the rest accumulates) is zeroed here.
+    ``dc``: split SH input (gsb_backward_split_sh); ``sh`` is the rest, grads["dc"] / grads["shs"] receive their gradients."""
     if accumulate and accumulate_means2D is False and grads.get("means2D") is not None:
         grads["means2D"].zero_()
     dev = means3D.device
@@ -516,18 +580,24 @@ def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rot
     with _device_ctx(dev):
         keep = []
         cs = _c_settings(rs, pack["sh_coeffs"], keep)
-        ci = _c_inputs(P, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+        ci = _c_inputs(P, means3D, sh if dc is None else None, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
         g = _Grads()
         g.dL_dmeans3D, g.dL_dmeans2D = _ptr(grads.get("means3D")), _ptr(grads.get("means2D"))
-        g.dL_dshs, g.dL_dcolors = _ptr(grads.get("shs")), _ptr(grads.get("colors_precomp"))
+        g.dL_dshs, g.dL_dcolors = _ptr(grads.get("shs")) if dc is None else None, _ptr(grads.get("colors_precomp"))
         g.dL_dopacities = _ptr(grads.get("opacities"))
         g.dL_dscales, g.dL_drotations = _ptr(grads.get("scales")), _ptr(grads.get("rotations"))
         g.dL_dcov3D = _ptr(grads.get("cov3D_precomp"))
         stream = _current_stream(dev)
         arena = _Arena(dev, stream)
-        rc = _C.gsb_backward(byref(cs), byref(ci), byref(pack["state"]), out_color.data_ptr(), out_invdepth.data_ptr(),
-                             grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), int(bool(accumulate)), arena.cb,
-                             None, stream)
+        if dc is None:
+            rc = _C.gsb_backward(byref(cs), byref(ci), byref(pack["state"]), out_color.data_ptr(), out_invdepth.data_ptr(),
+                                 grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), int(bool(accumulate)), arena.cb,
+                                 None, stream)
+        else:
+            sp = _split_sh(dc, sh, grads)
+            rc = _C.gsb_backward_split_sh(byref(cs), byref(ci), byref(sp), byref(pack["state"]), out_color.data_ptr(),
+                                          out_invdepth.data_ptr(), grad_color.data_ptr(), _ptr(grad_invdepth), byref(g),
+                                          int(bool(accumulate)), arena.cb, None, stream)
         _check(rc, arena)
 
 
@@ -633,32 +703,39 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings):
+                        raster_settings, dc=None):
+    """``dc`` (optional): split SH input -- ``dc`` [P,1,3] holds the DC coefficient and ``sh`` [P,M-1,3] the others (M-1 may
+    be 0); the result equals that of ``sh = cat((dc, sh), 1)`` without the concatenation."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings)
+                                     cov3Ds_precomp, raster_settings, dc)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings):
+                raster_settings, dc=None):
         args = [_f32c(means3D), _f32c(sh), _f32c(colors_precomp), _f32c(opacities), _f32c(scales), _f32c(rotations),
                 _f32c(cov3Ds_precomp)]
         if args[0] is None:  # P == 0
             args[0] = means3D.float().contiguous()
+        dcc = _f32c(dc)       # None also when P == 0: nothing to stage, the joint call renders the background
+        if dcc is not None and dcc.numel() != 3 * int(args[0].shape[0]):
+            raise ValueError(f"dc must hold one RGB coefficient per gaussian ([P,1,3]); got shape {tuple(dc.shape)}")
         try:
-            color, radii, invdepth, pack = _forward_impl(*args, raster_settings)
+            color, radii, invdepth, pack = _forward_impl(*args, raster_settings, dc=dcc)
         except Exception:
             if raster_settings.debug:
-                torch.save([a.detach().cpu() if a is not None else None for a in args], "snapshot_fw.dump")
+                dump = args + ([dcc] if dc is not None else [])
+                torch.save([a.detach().cpu() if a is not None else None for a in dump], "snapshot_fw.dump")
                 print("\nAn error occured in forward. Writing snapshot_fw.dump for debugging.")
             raise
         ctx.set_materialize_grads(False)   # an unused inverse-depth output reaches backward as None, not zeros
         ctx.raster_settings = raster_settings
         ctx.pack = pack
         ctx.shapes = dict(means2D=None if means2D is None else tuple(means2D.shape), opacities=tuple(opacities.shape),
-                          sh=None if sh is None else tuple(sh.shape))
-        ctx.save_for_backward(*[a if a is not None else torch.empty(0) for a in args], color, invdepth)
+                          sh=None if sh is None else tuple(sh.shape), dc=None if dc is None else tuple(dc.shape))
+        ctx.save_for_backward(*[a if a is not None else torch.empty(0) for a in args], color, invdepth,
+                              dcc if dcc is not None else torch.empty(0))
         ctx.mark_non_differentiable(radii)
         return color, radii, invdepth
 
@@ -668,6 +745,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         saved = [t if t.numel() > 0 else None for t in ctx.saved_tensors[:7]]
         means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp = saved
         out_color, out_invdepth = ctx.saved_tensors[7], ctx.saved_tensors[8]
+        dc = ctx.saved_tensors[9] if ctx.saved_tensors[9].numel() > 0 else None
         if means3D is None:
             means3D = ctx.saved_tensors[0]
         dev = means3D.device
@@ -676,6 +754,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         grads = dict(means3D=new(P, 3), means2D=new(P, 3), opacities=new(P))
         if sh is not None:
             grads["shs"] = new(*sh.shape)
+        if ctx.shapes["dc"] is not None:
+            grads["dc"] = new(*ctx.shapes["dc"])
+            if sh is None and ctx.shapes["sh"] is not None:     # rest without coefficients (SH degree 0 model)
+                grads["shs"] = torch.zeros(ctx.shapes["sh"], dtype=torch.float32, device=dev)
         if colors_precomp is not None:
             grads["colors_precomp"] = new(P, 3)
         if cov3Ds_precomp is not None:
@@ -684,23 +766,26 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads["scales"] = new(P, 3)
             grads["rotations"] = new(P, 4)
         if grad_out_color is None and grad_out_depth is None:
-            return (None,) * 9
+            return (None,) * 10
         gc = _f32c(grad_out_color)
         if gc is None:
             gc = torch.zeros((3, int(rs.image_height), int(rs.image_width)), dtype=torch.float32, device=dev)
         gd = _f32c(grad_out_depth)
+        if dc is None and "dc" in grads:                         # P == 0
+            grads["dc"].zero_()
         try:
             _backward_impl(ctx.pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                           out_color, out_invdepth, gc, gd, grads, accumulate=False)
+                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc)
         except Exception:
             if rs.debug:
-                torch.save([t.detach().cpu() for t in ctx.saved_tensors] + [gc.cpu()], "snapshot_bw.dump")
+                split = [ctx.saved_tensors[9].cpu()] if ctx.shapes["dc"] is not None else []
+                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()], "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
             raise
         g_op = grads["opacities"].reshape(ctx.shapes["opacities"])
         return (grads["means3D"], grads["means2D"] if ctx.shapes["means2D"] is not None else None, grads.get("shs"),
                 grads.get("colors_precomp"), g_op, grads.get("scales"), grads.get("rotations"),
-                grads.get("cov3D_precomp"), None)
+                grads.get("cov3D_precomp"), None, grads.get("dc"))
 
 
 class GaussianRasterizer(nn.Module):
@@ -724,12 +809,22 @@ class GaussianRasterizer(nn.Module):
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None):
+                cov3D_precomp=None, dc=None):
+        """``dc``: the split SH input of the accel branch (gaussian_renderer/__init__.py:90-100) -- ``dc`` [P,1,3] is the DC
+        coefficient and ``shs`` [P,M-1,3] the others (may have zero coefficients); gradients come back in the same split."""
         rs = self.raster_settings
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
         if ((scales is None or rotations is None) and cov3D_precomp is None) or \
                 ((scales is not None or rotations is not None) and cov3D_precomp is not None):
             raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
+        if dc is not None and colors_precomp is not None:
+            raise Exception("dc is the SH DC coefficient: it goes with shs, not with precomputed colors!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   rs)
+                                   rs, dc)
+
+
+# SparseGaussianAdam: bound here only on request (module docstring); sparse_adam.py is importable either way
+if os.environ.get("GSB_SPARSE_ADAM") == "1":
+    from .sparse_adam import SparseGaussianAdam  # noqa: E402,F401
+    __all__.append("SparseGaussianAdam")

@@ -72,7 +72,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     else:
         scales, rotations = pc.get_scaling, pc.get_rotation
 
-    shs = colors_precomp = None
+    shs = colors_precomp = dc = None
     if override_color is None:
         if getattr(pipe, "convert_SHs_python", False):
             feats = pc.get_features
@@ -81,8 +81,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             dir_pp = dir_pp / dir_pp.norm(dim=1, keepdim=True)
             colors_precomp = torch.clamp_min(_eval_sh(pc.active_sh_degree, shs_view, dir_pp) + 0.5, 0.0)
         elif separate_sh:
-            # the H100 rasterizer takes one [P,K,3] tensor; the split layout of the accel branch is re-joined here
-            shs = torch.cat((pc.get_features_dc, pc.get_features_rest), dim=1)
+            # the split layout of the accel branch: the rasterizer stages both tensors itself (no [P,M,3] concatenation)
+            dc, shs = pc.get_features_dc, pc.get_features_rest
         else:
             shs = pc.get_features
     else:
@@ -90,7 +90,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     rendered_image, radii, depth_image = rasterizer(
         means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors_precomp, opacities=pc.get_opacity,
-        scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp)
+        scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, dc=dc)
 
     if use_trained_exp:
         exposure = pc.get_exposure_from_name(viewpoint_camera.image_name)

@@ -146,6 +146,25 @@ int32_t gsb_backward(const GsbSettings *settings, const GsbInputs *in, const Gsb
                      const float *dL_dinvdepth, const GsbGrads *grads, int32_t accumulate,
                      gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
 
+/* Split SH input: the DC coefficient and the remaining ones in two tensors (GaussianRasterizer.forward(dc=..., shs=...),
+ * what scene.GaussianModel keeps as _features_dc / _features_rest), so no [P,M,3] concatenation is needed per view.
+ *   dc [P,1,3];  rest [P,M-1,3], or NULL when M == 1;  settings->sh_coeffs = M counts both;  in->shs must be NULL.
+ * Backward: dL_ddc [P,1,3] and dL_drest [P,M-1,3] receive the SH gradient (either may be NULL); grads->dL_dshs must be
+ * NULL.  Single-view calls only; results are those of gsb_forward / gsb_backward on the concatenated tensor. */
+typedef struct GsbSplitSH {
+    const float *dc;
+    const float *rest;
+    float *dL_ddc;
+    float *dL_drest;
+} GsbSplitSH;
+int32_t gsb_forward_split_sh(const GsbSettings *settings, const GsbInputs *in, const GsbSplitSH *split, float *out_color,
+                             int32_t *out_radii, float *out_invdepth, int64_t capacity_hint, gsb_alloc_fn alloc,
+                             void *alloc_ctx, GsbState *state_out, void *cuda_stream);
+int32_t gsb_backward_split_sh(const GsbSettings *settings, const GsbInputs *in, const GsbSplitSH *split, const GsbState *state,
+                              const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                              const float *dL_dinvdepth, const GsbGrads *grads, int32_t accumulate,
+                              gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
+
 /* View-batch variants (DESIGN.md section 5): V <= 16 cameras of equal image size against the SAME gaussians.
  * The per-gaussian parameters are read once for all views (preprocess), the V depth sorts / scans / tile sorts
  * run as single batched launches, and there is ONE host read-back (V instance counts) per call.
@@ -270,6 +289,25 @@ typedef struct GsbAdamArgs {
  * groups in one launch, with the activation backward (autograd's part in the reference) and the re-activation fused in:
  *   g_raw = J_act^T g;  m += (1-b1)(g_raw - m);  v = b2 v + (1-b2) g_raw^2;  p -= step_size * m / (sqrt(v)/bias2_sqrt + eps) */
 int32_t gsb_adam_step(const GsbAdamArgs *args, void *cuda_stream);
+
+/* SparseGaussianAdam (train.py --optimizer_type sparse_adam) over separate per-parameter tensors: every group is [N, width]
+ * row-major, float32, contiguous; param / grad / exp_avg / exp_avg_sq of one group share the layout.  Rows with
+ * visible[i] == 0 are neither read nor written.  Visible rows take the update of gsb_adam_step with step_size = lr and
+ * bias2_sqrt = 1 (no bias correction):
+ *   m += (1-b1)(g - m);  v = b2 v + (1-b2) g^2;  p -= lr * m / (sqrt(v) + eps)
+ * One launch for 1..GSB_MAX_SPARSE_GROUPS groups; no host synchronisation. */
+#define GSB_MAX_SPARSE_GROUPS 8
+typedef struct GsbSparseAdamGroup {
+    float *param;
+    const float *grad;
+    float *exp_avg;
+    float *exp_avg_sq;
+    int32_t width;            /* floats per row (> 0) */
+    float lr;
+    float eps;
+} GsbSparseAdamGroup;
+int32_t gsb_sparse_adam_step(const GsbSparseAdamGroup *groups, int32_t n_groups, const uint8_t *visible, int64_t N,
+                             float beta1, float beta2, void *cuda_stream);
 
 /* act <- activations of the store (after initialisation, densification or an opacity reset) */
 int32_t gsb_activate(int64_t P, int32_t sh_coeffs, const float *params, float *act, void *cuda_stream);
