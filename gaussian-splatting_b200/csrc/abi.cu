@@ -141,6 +141,22 @@ static int check_inputs(const GsbSettings *s, const GsbInputs *in, const GsbSpli
     return GSB_OK;
 }
 
+// camera gradient outputs: NULL (or every field NULL) = not requested; a requested output must be a 4-byte aligned pointer
+static int check_cam_grads(const char *fn, const GsbCameraGrads *cg, bool &want) {
+    want = false;
+    if (!cg) return GSB_OK;
+    float *const outs[4] = {cg->dL_dviewmatrix, cg->dL_dprojmatrix, cg->dL_dcampos, cg->dL_dbg};
+    for (float *p : outs) {
+        if (!p) continue;
+        if (reinterpret_cast<size_t>(p) & 3) {
+            set_error("%s: camera gradient outputs must be 4-byte aligned float pointers", fn);
+            return GSB_ERR_ARGUMENT;
+        }
+        want = true;
+    }
+    return GSB_OK;
+}
+
 static void *do_alloc(gsb_alloc_fn alloc, void *ctx, int which, size_t bytes) {
     void *p = alloc(ctx, which, bytes < 256 ? 256 : bytes);
     if (!p) set_error("allocator returned NULL for buffer %d (%zu bytes)", which, bytes);
@@ -370,10 +386,33 @@ int32_t gsb_forward_split_sh(const GsbSettings *s, const GsbInputs *in, const Gs
                         cuda_stream);
 }
 
-// shared body of gsb_backward (split == NULL) and gsb_backward_split_sh
+// Camera-gradient scratch of a K8 launch over P gaussians and V views: the warp partials and the dL/dbg partials.  Fills the
+// scratch pointers of `r` and returns the caller's PreBwdArgs::cam_part.
+static float *carve_cam_scratch(gsb_alloc_fn alloc, void *alloc_ctx, int V, int P, CamReduceArgs &r) {
+    r.V = V;
+    r.nslots = (int)cam_slots(P);
+    auto carve = [&](Carver &c) {
+        r.part = c.take<float>((size_t)V * CAM_TERMS * (r.nslots > 0 ? r.nslots : 1));
+        r.bg_part = c.take<float>((size_t)V * 3 * CAM_BG_BLOCKS);
+    };
+    Carver c0(nullptr);
+    carve(c0);
+    void *scr = do_alloc(alloc, alloc_ctx, GSB_BUF_SCRATCH1, c0.bytes());
+    if (!scr) return nullptr;
+    Carver c1(scr);
+    carve(c1);
+    return r.part;
+}
+
+static void set_cam_outputs(const GsbCameraGrads *cg, CamReduceArgs &r) {
+    r.dview = cg->dL_dviewmatrix; r.dproj = cg->dL_dprojmatrix; r.dcampos = cg->dL_dcampos; r.dbg = cg->dL_dbg;
+}
+
+// shared body of gsb_backward (split == NULL), gsb_backward_split_sh and gsb_backward_camera (cam_grads != NULL)
 static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
                          const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
-                         const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {
+                         const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream,
+                         const GsbCameraGrads *cam_grads = nullptr) {
     if (!s || !in || !st || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc) {
         set_error("%s: NULL argument", fn);
         return GSB_ERR_ARGUMENT;
@@ -385,6 +424,9 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
     if (rc) return rc;
     rc = check_inputs(s, in, split);
     if (rc) return rc;
+    bool want_cam = false;
+    rc = check_cam_grads(fn, cam_grads, want_cam);
+    if (rc) return rc;
     if (split && grads->dL_dshs) {
         set_error("%s: grads->dL_dshs must be NULL (dL_ddc / dL_drest receive the SH gradient)", fn);
         return GSB_ERR_ARGUMENT;
@@ -394,7 +436,14 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
         set_error("%s: state does not match the inputs (P %d vs %d)", fn, P, st->P);
         return GSB_ERR_ARGUMENT;
     }
-    if (P == 0) return GSB_OK;
+    CamReduceArgs cr;
+    memset(&cr, 0, sizeof(cr));
+    if (want_cam) {
+        if (!carve_cam_scratch(alloc, alloc_ctx, 1, P, cr)) return GSB_ERR_ALLOC;
+        set_cam_outputs(cam_grads, cr);
+        cr.final_T = st->final_T; cr.sv_image = 0; cr.npix = (size_t)cam.W * cam.H; cr.dL_dcolor = dL_dcolor;
+    }
+    if (P == 0) return want_cam ? launch_camera_grad_reduce(cr, accumulate != 0, debug, stream) : GSB_OK;
     const size_t dacc_bytes = align_up((size_t)P * DACC_STRIDE * sizeof(float), 256);
     float *dacc = static_cast<float *>(do_alloc(alloc, alloc_ctx, GSB_BUF_SCRATCH0, dacc_bytes));
     if (!dacc) return GSB_ERR_ALLOC;
@@ -420,7 +469,10 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
     if (split) pa.g.dL_dshs = split->dL_ddc;
     pa.p_begin = 0; pa.p_end = P;
     pa.peer.world = 0;
-    return launch_preprocess_bwd(cam, pa, split != nullptr, accumulate != 0, debug, stream);
+    pa.cam_part = want_cam ? cr.part : nullptr;
+    rc = launch_preprocess_bwd(cam, pa, split != nullptr, accumulate != 0, debug, stream);
+    if (rc || !want_cam) return rc;
+    return launch_camera_grad_reduce(cr, accumulate != 0, debug, stream);
 }
 
 int32_t gsb_backward(const GsbSettings *s, const GsbInputs *in, const GsbState *st, const float *out_color,
@@ -438,6 +490,14 @@ int32_t gsb_backward_split_sh(const GsbSettings *s, const GsbInputs *in, const G
     if (!split) { set_error("gsb_backward_split_sh: NULL argument"); return GSB_ERR_ARGUMENT; }
     return backward_impl("gsb_backward_split_sh", s, in, split, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads,
                          accumulate, alloc, alloc_ctx, cuda_stream);
+}
+
+int32_t gsb_backward_camera(const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
+                            const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
+                            const GsbGrads *grads, const GsbCameraGrads *cam_grads, int32_t accumulate, gsb_alloc_fn alloc,
+                            void *alloc_ctx, void *cuda_stream) {
+    return backward_impl("gsb_backward_camera", s, in, split, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate,
+                         alloc, alloc_ctx, cuda_stream, cam_grads);
 }
 
 static int check_batch(int32_t V, const GsbSettings *s, const GsbInputs *in, CamArgsBatch &cb) {
@@ -653,9 +713,13 @@ int32_t gsb_forward_batch_async(int32_t V, const GsbSettings *s, const GsbInputs
 static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs *in, const GsbState *states, const float *out_color,
                                const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth, const GsbGrads *grads,
                                int32_t accumulate, int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx, gsb_alloc_fn alloc,
-                               void *alloc_ctx, cudaStream_t stream, const GsbPeerTable *peers = nullptr) {
+                               void *alloc_ctx, cudaStream_t stream, const GsbPeerTable *peers = nullptr,
+                               const GsbCameraGrads *cam_grads = nullptr) {
     CamArgsBatch cb;
     int rc = check_batch(V, s, in, cb);
+    if (rc) return rc;
+    bool want_cam = false;
+    rc = check_cam_grads("gsb_backward_batch_camera", cam_grads, want_cam);
     if (rc) return rc;
     const bool debug = s[0].debug != 0;
     const CamArgs &c0 = cb.cam[0];
@@ -701,6 +765,21 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
     pa.cov_pre = nullptr; pa.splat = static_cast<const float4 *>(states[0].splat); pa.dacc = dacc; pa.g = *grads;
     pa.rest = nullptr; pa.dL_drest = nullptr;
     pa.peer.world = 0;
+    pa.cam_part = nullptr;
+    CamReduceArgs cr;
+    memset(&cr, 0, sizeof(cr));
+    if (want_cam) {
+        // the per-view sums cover every gaussian: one K8 launch, in this rank's process
+        if (peers || n_chunks > 1) {
+            set_error("camera gradients: not available on the chunked or peer backward (the sum would span chunks or ranks)");
+            return GSB_ERR_ARGUMENT;
+        }
+        if (!carve_cam_scratch(alloc, alloc_ctx, V, P, cr)) return GSB_ERR_ALLOC;
+        set_cam_outputs(cam_grads, cr);
+        cr.final_T = states[0].final_T; cr.sv_image = V > 1 ? (size_t)(states[1].final_T - states[0].final_T) : 0;
+        cr.npix = npix; cr.dL_dcolor = dL_dcolor;
+        pa.cam_part = cr.part;
+    }
     if (peers) {
         if (peers->world < 1 || peers->world > GSB_MAX_PEERS || peers->rank < 0 || peers->rank >= peers->world ||
             (int64_t)peers->rows_per_rank * peers->world < P) {
@@ -724,7 +803,7 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
         if (rc) return rc;
         if (on_chunk) on_chunk(chunk_ctx, c, pa.p_begin, pa.p_end);
     }
-    return GSB_OK;
+    return want_cam ? launch_camera_grad_reduce(cr, accumulate != 0, debug, stream) : GSB_OK;
 }
 
 int32_t gsb_backward_batch(int32_t V, const GsbSettings *s, const GsbInputs *in, const GsbState *states, const float *out_color,
@@ -736,6 +815,18 @@ int32_t gsb_backward_batch(int32_t V, const GsbSettings *s, const GsbInputs *in,
     }
     return backward_batch_impl(V, s, in, states, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate, 1, nullptr, nullptr,
                                alloc, alloc_ctx, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int32_t gsb_backward_batch_camera(int32_t V, const GsbSettings *s, const GsbInputs *in, const GsbState *states, const float *out_color,
+                                  const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth, const GsbGrads *grads,
+                                  const GsbCameraGrads *cam_grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx,
+                                  void *cuda_stream) {
+    if (!s || !in || !states || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc || in->P <= 0) {
+        set_error("gsb_backward_batch_camera: NULL argument or empty input");
+        return GSB_ERR_ARGUMENT;
+    }
+    return backward_batch_impl(V, s, in, states, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate, 1, nullptr, nullptr,
+                               alloc, alloc_ctx, static_cast<cudaStream_t>(cuda_stream), nullptr, cam_grads);
 }
 
 int32_t gsb_backward_batch_peer(int32_t V, const GsbSettings *s, const GsbInputs *in, const GsbState *states, const float *out_color,

@@ -54,7 +54,26 @@ struct PreBwdArgs {
     PeerTable peer;       // world > 0: outputs are ADDED into the owners' buffers (view-batch kernel, TMA rows only)
     const float *rest;    // split SH input: shs = DC rows, g.dL_dshs = their gradient, rest / dL_drest the other coefficients
     float *dL_drest;
+    float *cam_part;      // non-NULL: camera gradient requested; per-warp partials [V][CAM_TERMS][cam_slots(p_end - p_begin)]
 };
+
+// Camera gradient (gsb_backward_camera / gsb_backward_batch_camera): the 27 per-gaussian terms of preprocess.cu's CamGrad
+// (viewmatrix rows 0..3 x columns 0..2, projmatrix rows 0..3 x columns 0, 1, 3, campos), summed per warp by K8 and then over
+// the warps by camera_grad_reduce_kernel.  dL/dbg = sum over pixels of final_T * dL/dcolor: CAM_BG_BLOCKS partials per view
+// and channel (camera_bg_partial_kernel), summed by the same reduce kernel.  No float atomics: every sum has a fixed order.
+constexpr int CAM_TERMS = 27;
+constexpr int CAM_OUTPUTS = 16 + 16 + 3 + 3;
+constexpr int CAM_BG_BLOCKS = 128;
+struct CamReduceArgs {
+    int V, nslots;               // views; warp partials per view (0: no gaussians)
+    float *part;                 // [V][CAM_TERMS][nslots]
+    float *bg_part;              // [V][3][CAM_BG_BLOCKS] scratch
+    float *dview, *dproj, *dcampos, *dbg;   // [V][16], [V][16], [V][3], [V][3]; NULL = not requested
+    const float *final_T;        // view v: final_T + v * sv_image, [npix]
+    size_t sv_image, npix;
+    const float *dL_dcolor;      // [V][3][npix]
+};
+size_t cam_slots(int n_gauss);   // warp partials of one view for a K8 launch over n_gauss gaussians
 
 struct BinArgs {
     int P;
@@ -107,6 +126,7 @@ int launch_preprocess_fwd_batch(const CamArgsBatch &cb, const PreFwdArgs &a, con
 int launch_preprocess_bwd_batch(const CamArgsBatch &cb, const PreBwdArgs &a, const PreBwdBatchStrides &st, bool accumulate, bool debug,
                                 cudaStream_t stream);
 int launch_mark_visible(int P, const float *means, const float *view, uint8_t *present, cudaStream_t stream);
+int launch_camera_grad_reduce(const CamReduceArgs &r, bool accumulate, bool debug, cudaStream_t stream);
 
 size_t scan_partials_count(int P);
 // V > 1: blockIdx.y = view, arrays offset by the BinArgs strides; totals / n_dev are arrays of V counts

@@ -493,12 +493,43 @@ struct ViewGrad {
     float gm[3], g_m2[2], g_op, g_rgb[3], g_sc[3], g_rot[4], dS[6], d_rgb_sh[3], bas[16];
 };
 
+// One gaussian's contribution to the camera gradient (CAMGRAD instantiations), x~ = [x, y, z, 1]:
+//   t[3r + c]       dL/dV[r][c],  r < 4, c < 3   (column 3 of the viewmatrix is never read: its gradient is 0)
+//   t[12 + 3r + k]  dL/dPM[r][c], r < 4, c = 0, 1, 3 for k = 0, 1, 2   (column 2 is never read)
+//   t[24 + c]       dL/dcampos[c]
+struct CamGrad {
+    float t[CAM_TERMS];
+};
+
+__device__ __forceinline__ void cam_zero(CamGrad &cg) {
+#pragma unroll
+    for (int k = 0; k < CAM_TERMS; ++k) cg.t[k] = 0.f;
+}
+
+// Warp sum of the 27 terms (xor butterfly: a fixed order, every lane ends with the sum); lane 0 writes the warp's partial to
+// column `slot` of the [CAM_TERMS][nslots] panel.  Every lane of the warp must call this.
+__device__ __forceinline__ void cam_warp_partial(CamGrad &cg, float *panel, const int nslots, const int slot) {
+#pragma unroll
+    for (int k = 0; k < CAM_TERMS; ++k) {
+        float s = cg.t[k];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+        cg.t[k] = s;
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < CAM_TERMS; ++k) panel[(size_t)k * nslots + slot] = cg.t[k];
+    }
+}
+
 // K8 for one gaussian and one view: chain rule from the blend kernel's accumulators (mean2D / conic or raw moments, opacity,
 // rgb, inverse depth) to the rasterizer inputs.  Every field of `o` is written.
 // Returns false when the gaussian received no gradient in this view (all fields of `o` are zero then).
-template <bool VEC>
+// CAMGRAD: `*cg` receives the gaussian's camera gradient terms (all zero when it returns false).
+template <bool VEC, bool CAMGRAD = false>
 __device__ __forceinline__ bool preprocess_bwd_view(const CamParams &cam, const PreBwdArgs &a, const int i, const float *sh_row,
-                                                    const uint32_t bits, ViewGrad &o) {
+                                                    const uint32_t bits, ViewGrad &o, CamGrad *cg = nullptr) {
+    if (CAMGRAD) cam_zero(*cg);
     float (&gm)[3] = o.gm; float (&g_m2)[2] = o.g_m2; float &g_op = o.g_op; float (&g_rgb)[3] = o.g_rgb;
     float (&g_sc)[3] = o.g_sc; float (&g_rot)[4] = o.g_rot; float (&dS)[6] = o.dS; float (&d_rgb_sh)[3] = o.d_rgb_sh;
     float (&bas)[16] = o.bas;
@@ -550,6 +581,9 @@ __device__ __forceinline__ bool preprocess_bwd_view(const CamParams &cam, const 
             sh_dir_grad<VEC>(sh_row, d_rgb_sh, bx, by, bz, nb, ddx, ddy, ddz);
             const float dot = ux * ddx + uy * ddy + uz * ddz;
             gm[0] += (ddx - ux * dot) * inv; gm[1] += (ddy - uy * dot) * inv; gm[2] += (ddz - uz * dot) * inv;
+            if (CAMGRAD) {   // the view direction is mean - campos: campos takes minus this part of dL/dmean
+                cg->t[24] = -(ddx - ux * dot) * inv; cg->t[25] = -(ddy - uy * dot) * inv; cg->t[26] = -(ddz - uz * dot) * inv;
+            }
         } else {
             g_rgb[0] = d_rgb[0]; g_rgb[1] = d_rgb[1]; g_rgb[2] = d_rgb[2];
         }
@@ -603,6 +637,7 @@ __device__ __forceinline__ bool preprocess_bwd_view(const CamParams &cam, const 
         const float SM1[3] = {S0[0] * M1[0] + S0[1] * M1[1] + S0[2] * M1[2], S1[0] * M1[0] + S1[1] * M1[1] + S1[2] * M1[2],
                               S2[0] * M1[0] + S2[1] * M1[1] + S2[2] * M1[2]};
         float dJ00 = 0.f, dJ02 = 0.f, dJ11 = 0.f, dJ12 = 0.f;
+        float dMv0[3], dMv1[3];   // dL/dM (CAMGRAD only)
         const float *v = cam.view;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
@@ -610,6 +645,7 @@ __device__ __forceinline__ bool preprocess_bwd_view(const CamParams &cam, const 
             const float dM1 = 2.f * dL_dc * SM1[c] + dL_db * SM0[c];
             dJ00 += dM0 * v[4 * c + 0]; dJ02 += dM0 * v[4 * c + 2];
             dJ11 += dM1 * v[4 * c + 1]; dJ12 += dM1 * v[4 * c + 2];
+            if (CAMGRAD) { dMv0[c] = dM0; dMv1[c] = dM1; }
         }
         const float tz = cv.tz, tz2 = 1.0f / (tz * tz), tz3 = tz2 / tz;
         const float fx = cam.focal_x, fy = cam.focal_y;
@@ -619,6 +655,20 @@ __device__ __forceinline__ bool preprocess_bwd_view(const CamParams &cam, const 
         dtz -= d_invd * tz2;
 #pragma unroll
         for (int c = 0; c < 3; ++c) gm[c] += dtx * v[4 * c + 0] + dty * v[4 * c + 1] + dtz * v[4 * c + 2];
+        const float xt[4] = {px, py, pz, 1.0f};
+        if (CAMGRAD) {
+            // p_view = x~ V: dL/dV[r][c] = x~_r dL/dp_view[c].  M = J Rw2c with Rw2c[k][c] = V[c][k] adds
+            // dL/dV[c][k] += sum_i dL/dM[i][c] J[i][k] on the rotation block (J01 = J10 = 0, J's tx / ty are the clamped ones)
+            const float J00 = fx / tz, J02 = -(fx * cv.tx) / (tz * tz), J11 = fy / tz, J12 = -(fy * cv.ty) / (tz * tz);
+#pragma unroll
+            for (int r = 0; r < 4; ++r) { cg->t[3 * r] = xt[r] * dtx; cg->t[3 * r + 1] = xt[r] * dty; cg->t[3 * r + 2] = xt[r] * dtz; }
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                cg->t[3 * c] += dMv0[c] * J00;
+                cg->t[3 * c + 1] += dMv1[c] * J11;
+                cg->t[3 * c + 2] += dMv0[c] * J02 + dMv1[c] * J12;
+            }
+        }
 
         // NDC 2D mean -> 3D mean
         {
@@ -631,6 +681,14 @@ __device__ __forceinline__ bool preprocess_bwd_view(const CamParams &cam, const 
 #pragma unroll
             for (int c = 0; c < 3; ++c)
                 gm[c] += (pm[4 * c + 0] * pw - pm[4 * c + 3] * mul1) * d_m2x + (pm[4 * c + 1] * pw - pm[4 * c + 3] * mul2) * d_m2y;
+            if (CAMGRAD) {
+                // p_hom = x~ PM, ndc = p_hom.xy / (p_hom.w + eps): dL/dPM[r][c] = x~_r dL/dp_hom[c] for c = 0, 1, 3
+                const float gx = pw * d_m2x, gy = pw * d_m2y, gw = -(mul1 * d_m2x + mul2 * d_m2y);
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    cg->t[12 + 3 * r] = xt[r] * gx; cg->t[12 + 3 * r + 1] = xt[r] * gy; cg->t[12 + 3 * r + 2] = xt[r] * gw;
+                }
+            }
         }
 
         // Sigma -> scale, rotation
@@ -708,7 +766,8 @@ __device__ __forceinline__ T *shift_ptr(T *p, const long long bytes) {
 }
 
 // K8, one view.  SPLIT: split SH input and gradient (a.shs / a.g.dL_dshs = DC rows, a.rest / a.dL_drest = the rest; TMA false).
-template <bool ACC, bool TMA, bool SPLIT = false>
+// CAMGRAD: every warp also writes its sum of the camera gradient terms to a.cam_part ([CAM_TERMS][4 * gridDim.x]).
+template <bool ACC, bool TMA, bool SPLIT = false, bool CAMGRAD = false>
 __global__ void __launch_bounds__(PRE_THREADS)
 preprocess_bwd_kernel(const CamArgs ca, const PreBwdArgs a) {
     __shared__ CamParams cam;
@@ -731,7 +790,12 @@ preprocess_bwd_kernel(const CamArgs ca, const PreBwdArgs a) {
     const int M = cam.sh_coeffs;
     float *sh_row = sh_rows + threadIdx.x * sh_stride<TMA>(shn);
     ViewGrad g;
-    if (live) preprocess_bwd_view<TMA>(cam, a, i, sh_row, __float_as_uint(a.splat[(size_t)i * SPLAT_F4 + 2].w), g);
+    CamGrad cg;
+    if (live) preprocess_bwd_view<TMA, CAMGRAD>(cam, a, i, sh_row, __float_as_uint(a.splat[(size_t)i * SPLAT_F4 + 2].w), g, &cg);
+    if (CAMGRAD) {
+        if (!live) cam_zero(cg);
+        cam_warp_partial(cg, a.cam_part, PRE_THREADS / 32 * gridDim.x, blockIdx.x * (PRE_THREADS / 32) + threadIdx.x / 32);
+    }
 
     // SH gradient rows go out through shared memory (coalesced / one bulk store); each thread rewrites only its own row
     if ((a.g.dL_dshs || (SPLIT && a.dL_drest)) && a.shs) {
@@ -755,7 +819,8 @@ preprocess_bwd_kernel(const CamArgs ca, const PreBwdArgs a) {
 // View-batch K8: parameters read once, the V views' accumulators chained one after the other, the per-gaussian
 // gradient summed over views in registers (SH: in a second shared-memory row) and written ONCE.
 // Per-view arrays (dacc, splat, means2D gradient) are [V][...] with uniform strides.
-template <bool ACC, bool TMA>
+// CAMGRAD: view v's warp partials of the camera gradient go to panel v of a.cam_part ([V][CAM_TERMS][4 * gridDim.x]).
+template <bool ACC, bool TMA, bool CAMGRAD = false>
 __global__ void __launch_bounds__(PRE_THREADS)
 preprocess_bwd_batch_kernel(const CamArgsBatch cb, const PreBwdArgs a, const PreBwdBatchStrides st) {
     __shared__ CamParams cams[GSB_MAX_VIEWS];
@@ -781,6 +846,39 @@ preprocess_bwd_batch_kernel(const CamArgsBatch cb, const PreBwdArgs a, const Pre
     float gm[3] = {0.f, 0.f, 0.f}, g_op = 0.f, g_rgb[3] = {0.f, 0.f, 0.f}, g_sc[3] = {0.f, 0.f, 0.f};
     float g_rot[4] = {0.f, 0.f, 0.f, 0.f}, dS[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     const bool want_sh = a.g.dL_dshs && a.shs;
+    // view v of a live gaussian: its gradient added to the sums above (CAMGRAD: its camera terms written to *cg)
+    auto one_view = [&](const int v, CamGrad *cg) {
+        PreBwdArgs av = a;
+        av.splat += (size_t)v * st.splat; av.dacc += (size_t)v * st.dacc;
+        const uint32_t bits = __float_as_uint(av.splat[(size_t)i * SPLAT_F4 + 2].w);
+        if (!(bits & 8u)) {
+            if (a.g.dL_dmeans2D) {
+                float *m2 = a.g.dL_dmeans2D + (size_t)v * st.means2D + 3 * (size_t)i;
+                m2[0] = 0.f; m2[1] = 0.f; m2[2] = 0.f;
+            }
+            return;
+        }
+        ViewGrad g;
+        if (!preprocess_bwd_view<TMA, CAMGRAD>(cams[v], av, i, sh_row, bits, g, cg)) {
+            if (a.g.dL_dmeans2D) {
+                float *m2 = a.g.dL_dmeans2D + (size_t)v * st.means2D + 3 * (size_t)i;
+                m2[0] = 0.f; m2[1] = 0.f; m2[2] = 0.f;
+            }
+            return;
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { gm[c] += g.gm[c]; g_rgb[c] += g.g_rgb[c]; g_sc[c] += g.g_sc[c]; }
+#pragma unroll
+        for (int c = 0; c < 4; ++c) g_rot[c] += g.g_rot[c];
+#pragma unroll
+        for (int c = 0; c < 6; ++c) dS[c] += g.dS[c];
+        g_op += g.g_op;
+        if (want_sh) sh_grad_row<TMA, true>(gr, g.bas, g.d_rgb_sh, nb, M);
+        if (a.g.dL_dmeans2D) {
+            float *m2 = a.g.dL_dmeans2D + (size_t)v * st.means2D + 3 * (size_t)i;
+            m2[0] = g.g_m2[0]; m2[1] = g.g_m2[1]; m2[2] = 0.f;
+        }
+    };
     if (live) {
         if (want_sh) {
             if (TMA) {
@@ -795,38 +893,19 @@ preprocess_bwd_batch_kernel(const CamArgsBatch cb, const PreBwdArgs a, const Pre
 #else
         constexpr int kViewUnroll = 1;
 #endif
+        if (!CAMGRAD) {
 #pragma unroll kViewUnroll
+            for (int v = 0; v < cb.V; ++v) one_view(v, nullptr);
+        }
+    }
+    if (CAMGRAD) {
+        // every lane of the block runs every view (compute or zero, then the warp sum): no lane may skip a shuffle
+        const int nslots = PRE_THREADS / 32 * gridDim.x, slot = blockIdx.x * (PRE_THREADS / 32) + threadIdx.x / 32;
         for (int v = 0; v < cb.V; ++v) {
-            PreBwdArgs av = a;
-            av.splat += (size_t)v * st.splat; av.dacc += (size_t)v * st.dacc;
-            const uint32_t bits = __float_as_uint(av.splat[(size_t)i * SPLAT_F4 + 2].w);
-            if (!(bits & 8u)) {
-                if (a.g.dL_dmeans2D) {
-                    float *m2 = a.g.dL_dmeans2D + (size_t)v * st.means2D + 3 * (size_t)i;
-                    m2[0] = 0.f; m2[1] = 0.f; m2[2] = 0.f;
-                }
-                continue;
-            }
-            ViewGrad g;
-            if (!preprocess_bwd_view<TMA>(cams[v], av, i, sh_row, bits, g)) {
-                if (a.g.dL_dmeans2D) {
-                    float *m2 = a.g.dL_dmeans2D + (size_t)v * st.means2D + 3 * (size_t)i;
-                    m2[0] = 0.f; m2[1] = 0.f; m2[2] = 0.f;
-                }
-                continue;
-            }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) { gm[c] += g.gm[c]; g_rgb[c] += g.g_rgb[c]; g_sc[c] += g.g_sc[c]; }
-#pragma unroll
-            for (int c = 0; c < 4; ++c) g_rot[c] += g.g_rot[c];
-#pragma unroll
-            for (int c = 0; c < 6; ++c) dS[c] += g.dS[c];
-            g_op += g.g_op;
-            if (want_sh) sh_grad_row<TMA, true>(gr, g.bas, g.d_rgb_sh, nb, M);
-            if (a.g.dL_dmeans2D) {
-                float *m2 = a.g.dL_dmeans2D + (size_t)v * st.means2D + 3 * (size_t)i;
-                m2[0] = g.g_m2[0]; m2[1] = g.g_m2[1]; m2[2] = 0.f;
-            }
+            CamGrad cg;
+            cam_zero(cg);
+            if (live) one_view(v, &cg);
+            cam_warp_partial(cg, a.cam_part + (size_t)v * CAM_TERMS * nslots, nslots, slot);
         }
     }
     if (TMA && a.peer.world > 0) {
@@ -909,7 +988,18 @@ int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool split, bo
     const int grid = (int)ceil_div(a.p_end - a.p_begin, PRE_THREADS);
     const bool tma = !split && use_tma_rows(a.shs, a.g.dL_dshs, ca.sh_coeffs);
     const size_t smem = a.shs ? sh_smem_bytes(tma, ca.sh_coeffs, 1) : 0;
-    if (split) {
+    if (a.cam_part) {   // camera gradient: the accumulate switch only concerns the per-gaussian outputs here
+        if (split) {
+            if (accumulate) GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, false, true, true>), grid, smem, ca, a);
+            else GSB_PRE_LAUNCH((preprocess_bwd_kernel<false, false, true, true>), grid, smem, ca, a);
+        } else if (accumulate) {
+            if (tma) GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, true, false, true>), grid, smem, ca, a);
+            else GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, false, false, true>), grid, smem, ca, a);
+        } else {
+            if (tma) GSB_PRE_LAUNCH((preprocess_bwd_kernel<false, true, false, true>), grid, smem, ca, a);
+            else GSB_PRE_LAUNCH((preprocess_bwd_kernel<false, false, false, true>), grid, smem, ca, a);
+        }
+    } else if (split) {
         if (accumulate) GSB_PRE_LAUNCH((preprocess_bwd_kernel<true, false, true>), grid, smem, ca, a);
         else GSB_PRE_LAUNCH((preprocess_bwd_kernel<false, false, true>), grid, smem, ca, a);
     } else if (accumulate) {
@@ -950,13 +1040,114 @@ int launch_preprocess_bwd_batch(const CamArgsBatch &cb, const PreBwdArgs &a, con
         }
     }
     const size_t smem = a.shs ? sh_smem_bytes(tma, cb.cam[0].sh_coeffs, 2) : 0;
-    if (accumulate) {
+    if (a.cam_part) {
+        if (a.peer.world > 0) {
+            set_error("camera gradients are not available with peer gradients: their sum would have to span the ranks");
+            return GSB_ERR_ARGUMENT;
+        }
+        if (accumulate) {
+            if (tma) GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<true, true, true>), grid, smem, cb, a, st);
+            else GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<true, false, true>), grid, smem, cb, a, st);
+        } else {
+            if (tma) GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<false, true, true>), grid, smem, cb, a, st);
+            else GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<false, false, true>), grid, smem, cb, a, st);
+        }
+    } else if (accumulate) {
         if (tma) GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<true, true>), grid, smem, cb, a, st);
         else GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<true, false>), grid, smem, cb, a, st);
     } else {
         if (tma) GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<false, true>), grid, smem, cb, a, st);
         else GSB_PRE_LAUNCH((preprocess_bwd_batch_kernel<false, false>), grid, smem, cb, a, st);
     }
+    return GSB_OK;
+}
+
+// ---- camera gradient: the per-view sums ------------------------------------------------------------------------------------
+// One block per (output entry, view): the block sums its term's warp partials (or, for bg, final_T * dL/dcolor over the
+// pixels) with a strided per-thread loop and a shared-memory tree -- a fixed order, so the result is reproducible bit for bit.
+constexpr int CAM_RED_THREADS = 256;
+
+// output entry j (0..15 viewmatrix, 16..31 projmatrix, 32..34 campos) -> term of CamGrad, or -1 for a column the forward never reads
+__device__ __forceinline__ int cam_term_of(const int j) {
+    if (j < 16) return (j & 3) == 3 ? -1 : 3 * (j >> 2) + (j & 3);
+    if (j < 32) {
+        const int r = (j - 16) >> 2, c = (j - 16) & 3;
+        return c == 2 ? -1 : 12 + 3 * r + (c == 3 ? 2 : c);
+    }
+    return 24 + (j - 32);
+}
+
+// block-wide sum of s (shared-memory tree, fixed order); thread 0 writes it to *out (ACC: adds)
+__device__ __forceinline__ void block_sum_to(const float s, float *red, float *out, const bool acc) {
+    const int t = threadIdx.x;
+    red[t] = s;
+    __syncthreads();
+    for (int h = CAM_RED_THREADS / 2; h > 0; h >>= 1) {
+        if (t < h) red[t] += red[t + h];
+        __syncthreads();
+    }
+    if (t == 0) *out = acc ? *out + red[0] : red[0];
+    __syncthreads();   // red is reused by the caller's next sum
+}
+
+template <bool ACC>
+__global__ void __launch_bounds__(CAM_RED_THREADS)
+camera_grad_reduce_kernel(const CamReduceArgs r) {
+    __shared__ float red[CAM_RED_THREADS];
+    const int j = blockIdx.x, v = blockIdx.y, t = threadIdx.x;
+    float *out;
+    if (j < 16) out = r.dview ? r.dview + 16 * v + j : nullptr;
+    else if (j < 32) out = r.dproj ? r.dproj + 16 * v + (j - 16) : nullptr;
+    else if (j < 35) out = r.dcampos ? r.dcampos + 3 * v + (j - 32) : nullptr;
+    else out = r.dbg ? r.dbg + 3 * v + (j - 35) : nullptr;
+    if (!out) return;                      // uniform per block
+    float s = 0.f;
+    const float *p;
+    int n;
+    if (j < 35) {
+        const int term = cam_term_of(j);
+        if (term < 0) {
+            if (t == 0 && !ACC) *out = 0.f;
+            return;
+        }
+        p = r.part + ((size_t)v * CAM_TERMS + term) * r.nslots;
+        n = r.nslots;
+    } else {
+        p = r.bg_part + ((size_t)v * 3 + (j - 35)) * CAM_BG_BLOCKS;
+        n = CAM_BG_BLOCKS;
+    }
+    for (int k = t; k < n; k += CAM_RED_THREADS) s += p[k];
+    block_sum_to(s, red, out, ACC);
+}
+
+// dL/dbg partials: block b of view v sums final_T * dL/dcolor[c] over its contiguous pixel range, c = 0..2
+__global__ void __launch_bounds__(CAM_RED_THREADS)
+camera_bg_partial_kernel(const CamReduceArgs r) {
+    __shared__ float red[CAM_RED_THREADS];
+    const int b = blockIdx.x, v = blockIdx.y, t = threadIdx.x;
+    const size_t chunk = (r.npix + CAM_BG_BLOCKS - 1) / CAM_BG_BLOCKS;
+    const size_t p0 = b * chunk, p1 = min(r.npix, p0 + chunk);
+    const float *T = r.final_T + (size_t)v * r.sv_image;
+    for (int c = 0; c < 3; ++c) {
+        const float *g = r.dL_dcolor + ((size_t)v * 3 + c) * r.npix;
+        float s = 0.f;
+        for (size_t k = p0 + t; k < p1; k += CAM_RED_THREADS) s += T[k] * g[k];
+        block_sum_to(s, red, r.bg_part + ((size_t)v * 3 + c) * CAM_BG_BLOCKS + b, false);
+    }
+}
+
+size_t cam_slots(int n_gauss) { return (size_t)ceil_div(n_gauss > 0 ? n_gauss : 0, PRE_THREADS) * (PRE_THREADS / 32); }
+
+int launch_camera_grad_reduce(const CamReduceArgs &r, bool accumulate, bool debug, cudaStream_t stream) {
+    if (!r.dview && !r.dproj && !r.dcampos && !r.dbg) return GSB_OK;
+    if (r.dbg) {
+        const char *name = "camera_bg_partial";
+        GSB_LAUNCH(name, debug, stream, camera_bg_partial_kernel, dim3(CAM_BG_BLOCKS, r.V), CAM_RED_THREADS, 0, r);
+    }
+    const char *name = "camera_grad_reduce";
+    const dim3 grid(CAM_OUTPUTS, r.V);
+    if (accumulate) GSB_LAUNCH(name, debug, stream, camera_grad_reduce_kernel<true>, grid, CAM_RED_THREADS, 0, r);
+    else GSB_LAUNCH(name, debug, stream, camera_grad_reduce_kernel<false>, grid, CAM_RED_THREADS, 0, r);
     return GSB_OK;
 }
 

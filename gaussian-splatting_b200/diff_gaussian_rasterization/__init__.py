@@ -87,6 +87,10 @@ class _SplitSH(Structure):           # GsbSplitSH
     _fields_ = [("dc", c_void_p), ("rest", c_void_p), ("dL_ddc", c_void_p), ("dL_drest", c_void_p)]
 
 
+class _CameraGrads(Structure):       # GsbCameraGrads
+    _fields_ = [("dL_dviewmatrix", c_void_p), ("dL_dprojmatrix", c_void_p), ("dL_dcampos", c_void_p), ("dL_dbg", c_void_p)]
+
+
 class _SparseAdamGroup(Structure):   # GsbSparseAdamGroup
     _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p), ("width", c_int32),
                 ("lr", c_float), ("eps", c_float)]
@@ -115,6 +119,14 @@ def _load(path: Optional[str] = None):
     lib.gsb_backward_split_sh.restype = c_int32
     lib.gsb_backward_split_sh.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), POINTER(_State), c_void_p,
                                           c_void_p, c_void_p, c_void_p, POINTER(_Grads), c_int32, _ALLOC_FN, c_void_p, c_void_p]
+    lib.gsb_backward_camera.restype = c_int32
+    lib.gsb_backward_camera.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), POINTER(_State), c_void_p, c_void_p,
+                                        c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads), c_int32, _ALLOC_FN, c_void_p,
+                                        c_void_p]
+    lib.gsb_backward_batch_camera.restype = c_int32
+    lib.gsb_backward_batch_camera.argtypes = [c_int32, POINTER(_Settings), POINTER(_Inputs), POINTER(_State), c_void_p, c_void_p,
+                                              c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads), c_int32, _ALLOC_FN,
+                                              c_void_p, c_void_p]
     lib.gsb_sparse_adam_step.restype = c_int32
     lib.gsb_sparse_adam_step.argtypes = [POINTER(_SparseAdamGroup), c_int32, c_void_p, c_int64, c_float, c_float, c_void_p]
     lib.gsb_forward_batch.restype = c_int32
@@ -567,12 +579,36 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
     return color, radii, invdepth, pack
 
 
+CAMERA_KEYS = ("viewmatrix", "projmatrix", "campos", "bg")     # GsbCameraGrads, in field order
+_CAMERA_NUMEL = dict(viewmatrix=16, projmatrix=16, campos=3, bg=3)
+
+
+def _camera_grads(cam_grads: Optional[dict], V: Optional[int] = None):
+    """GsbCameraGrads over the float32 contiguous tensors of ``cam_grads`` (keys CAMERA_KEYS, missing / None = not requested),
+    each [16] / [3] per view ([V,16] / [V,3] for the view batch); None when nothing is requested."""
+    if not cam_grads or all(cam_grads.get(k) is None for k in CAMERA_KEYS):
+        return None
+    cg = _CameraGrads()
+    for k in CAMERA_KEYS:
+        t = cam_grads.get(k)
+        if t is None:
+            continue
+        n = _CAMERA_NUMEL[k] * (1 if V is None else V)
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n:
+            raise ValueError(f"camera gradient '{k}': contiguous float32 tensor of {n} elements expected, got "
+                             f"{t.dtype} {tuple(t.shape)}")
+        setattr(cg, "dL_d" + k, t.data_ptr())
+    return cg
+
+
 def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                    out_color, out_invdepth, grad_color, grad_invdepth, grads: dict, accumulate: bool,
-                   accumulate_means2D: Optional[bool] = None, dc=None):
+                   accumulate_means2D: Optional[bool] = None, dc=None, cam_grads: Optional[dict] = None):
     """grads: tensors to fill (accumulate=False) or add into (accumulate=True).  The C ABI has one accumulate
     switch; a per-view means2D buffer (accumulate_means2D=False while the rest accumulates) is zeroed here.
-    ``dc``: split SH input (gsb_backward_split_sh); ``sh`` is the rest, grads["dc"] / grads["shs"] receive their gradients."""
+    ``dc``: split SH input (gsb_backward_split_sh); ``sh`` is the rest, grads["dc"] / grads["shs"] receive their gradients.
+    ``cam_grads``: {"viewmatrix": [16], "projmatrix": [16], "campos": [3], "bg": [3]} float32 tensors (any subset) that receive
+    the camera gradient under the same accumulate switch (gsb_backward_camera)."""
     if accumulate and accumulate_means2D is False and grads.get("means2D") is not None:
         grads["means2D"].zero_()
     dev = means3D.device
@@ -589,7 +625,13 @@ def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rot
         g.dL_dcov3D = _ptr(grads.get("cov3D_precomp"))
         stream = _current_stream(dev)
         arena = _Arena(dev, stream)
-        if dc is None:
+        cg = _camera_grads(cam_grads)
+        if cg is not None:
+            sp = _split_sh(dc, sh, grads) if dc is not None else None
+            rc = _C.gsb_backward_camera(byref(cs), byref(ci), byref(sp) if sp is not None else None, byref(pack["state"]),
+                                        out_color.data_ptr(), out_invdepth.data_ptr(), grad_color.data_ptr(), _ptr(grad_invdepth),
+                                        byref(g), byref(cg), int(bool(accumulate)), arena.cb, None, stream)
+        elif dc is None:
             rc = _C.gsb_backward(byref(cs), byref(ci), byref(pack["state"]), out_color.data_ptr(), out_invdepth.data_ptr(),
                                  grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), int(bool(accumulate)), arena.cb,
                                  None, stream)
@@ -652,15 +694,22 @@ def capacity_for(count: int) -> int:
 
 
 def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, rotations, out_color, out_invdepth,
-                         grad_color, grad_invdepth, grads: dict, accumulate: bool, n_chunks: int = 1, on_chunk=None, peers=None):
+                         grad_color, grad_invdepth, grads: dict, accumulate: bool, n_chunks: int = 1, on_chunk=None, peers=None,
+                         cam_grads: Optional[dict] = None):
     """View-batch backward (gsb_backward_batch).  grads: tensors holding / receiving the gradient SUMMED over the views
     (means2D, if present, is [V,P,3] and per view).  ``n_chunks`` > 1: gsb_backward_batch_chunked -- the last kernel runs in
     gaussian-range chunks and ``on_chunk(chunk, p_begin, p_end)`` is called after each chunk has been enqueued (rows
     [p_begin, p_end) of every gradient are final in stream order from there on).  ``peers`` = (world, rank, rows_per_rank,
     [base pointers]): gsb_backward_batch_peer -- the gradients are ADDED into the owner ranks' buffers (fused reduce-scatter;
-    gaussian_renderer.peer.PeerGradientBucket drives the protocol around it)."""
+    gaussian_renderer.peer.PeerGradientBucket drives the protocol around it).  ``cam_grads``: {"viewmatrix": [V,16],
+    "projmatrix": [V,16], "campos": [V,3], "bg": [V,3]} float32 tensors (any subset) receiving each view's camera gradient
+    (gsb_backward_batch_camera); not with ``n_chunks`` > 1, ``on_chunk`` or ``peers``."""
     dev = means3D.device
     V, P = pack["V"], int(means3D.shape[0])
+    cg = _camera_grads(cam_grads, V)
+    if cg is not None and (peers is not None or n_chunks > 1 or on_chunk is not None):
+        raise ValueError("camera gradients are not available on the chunked or peer view-batch backward: the per-view sum "
+                         "would have to span gaussian chunks or ranks")
     with _device_ctx(dev):
         keep = []
         cs = (_Settings * V)(*[_c_settings(rs, pack["sh_coeffs"], keep) for rs in settings_list])
@@ -695,6 +744,11 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
             _check(rc, arena)
             if err:
                 raise err[0]
+        elif cg is not None:
+            rc = _C.gsb_backward_batch_camera(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
+                                              grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), byref(cg),
+                                              int(bool(accumulate)), arena.cb, None, stream)
+            _check(rc, arena)
         else:
             rc = _C.gsb_backward_batch(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
                                        grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), int(bool(accumulate)), arena.cb, None,
@@ -705,15 +759,28 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, dc=None):
     """``dc`` (optional): split SH input -- ``dc`` [P,1,3] holds the DC coefficient and ``sh`` [P,M-1,3] the others (M-1 may
-    be 0); the result equals that of ``sh = cat((dc, sh), 1)`` without the concatenation."""
+    be 0); the result equals that of ``sh = cat((dc, sh), 1)`` without the concatenation.
+
+    Camera gradients: when grad mode is on and any of ``raster_settings.viewmatrix`` / ``.projmatrix`` / ``.campos`` / ``.bg``
+    requires grad, the four tensors become trailing inputs of the autograd function and those that require grad receive
+    their gradient (gsb_backward_camera; conventions in include/gs_b200.h).  Otherwise the call is exactly the plain one."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings, dc)
+                                     cov3Ds_precomp, raster_settings, dc, *_camera_inputs(raster_settings))
+
+
+def _camera_inputs(rs) -> tuple:
+    """(viewmatrix, projmatrix, campos, bg) of the settings if grad mode is on and one of them requires grad, else ()."""
+    cams = tuple(getattr(rs, k) for k in CAMERA_KEYS)
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in cams):
+        return cams
+    return ()
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, dc=None):
+                raster_settings, dc=None, *camera):
+        # camera: the settings' (viewmatrix, projmatrix, campos, bg) as inputs of their own (rasterize_gaussians), or ()
         args = [_f32c(means3D), _f32c(sh), _f32c(colors_precomp), _f32c(opacities), _f32c(scales), _f32c(rotations),
                 _f32c(cov3Ds_precomp)]
         if args[0] is None:  # P == 0
@@ -737,6 +804,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.save_for_backward(*[a if a is not None else torch.empty(0) for a in args], color, invdepth,
                               dcc if dcc is not None else torch.empty(0))
         ctx.mark_non_differentiable(radii)
+        ctx.camera = [(tuple(t.shape), t.dtype) for t in camera]
         return color, radii, invdepth
 
     @staticmethod
@@ -765,8 +833,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         else:
             grads["scales"] = new(P, 3)
             grads["rotations"] = new(P, 4)
+        cam_grads = {k: torch.empty(_CAMERA_NUMEL[k], dtype=torch.float32, device=dev)
+                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[10 + j]}
         if grad_out_color is None and grad_out_depth is None:
-            return (None,) * 10
+            return (None,) * (10 + len(ctx.camera))
         gc = _f32c(grad_out_color)
         if gc is None:
             gc = torch.zeros((3, int(rs.image_height), int(rs.image_width)), dtype=torch.float32, device=dev)
@@ -775,17 +845,20 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads["dc"].zero_()
         try:
             _backward_impl(ctx.pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc)
+                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc, cam_grads=cam_grads)
         except Exception:
             if rs.debug:
                 split = [ctx.saved_tensors[9].cpu()] if ctx.shapes["dc"] is not None else []
-                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()], "snapshot_bw.dump")
+                camera = [getattr(rs, k).detach().cpu() for k in CAMERA_KEYS] if ctx.camera else []
+                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()] + camera, "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
             raise
         g_op = grads["opacities"].reshape(ctx.shapes["opacities"])
+        g_cam = tuple(cam_grads[k].view(shape).to(dtype) if k in cam_grads else None
+                      for k, (shape, dtype) in zip(CAMERA_KEYS, ctx.camera))
         return (grads["means3D"], grads["means2D"] if ctx.shapes["means2D"] is not None else None, grads.get("shs"),
                 grads.get("colors_precomp"), g_op, grads.get("scales"), grads.get("rotations"),
-                grads.get("cov3D_precomp"), None, grads.get("dc"))
+                grads.get("cov3D_precomp"), None, grads.get("dc")) + g_cam
 
 
 class GaussianRasterizer(nn.Module):

@@ -208,6 +208,11 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     gsb_backward_batch: the gaussians' parameters are read once for all views in the per-gaussian kernels, the
     depth sorts / scans / tile sorts of the views run as single batched launches, the summed gradient is written
     once, and there is ONE host read-back per chunk.  ``batched=False`` runs view by view (one read-back each).
+
+    A camera whose ``world_view_transform`` / ``full_proj_transform`` / ``camera_center`` (or ``bg_color``) requires grad
+    receives its gradient like a non-leaf gaussian input: each view's camera gradient comes out of the backward kernels
+    (gsb_backward_batch_camera / gsb_backward_camera) and is chained into the camera tensors' graphs at the end.  This is
+    not available with ``grad_chunks`` > 1, ``on_grad_chunk`` or ``peers`` (ValueError).
     """
     takes_grad_out = False
     if loss_returns_grad:
@@ -235,6 +240,26 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     c["opacities"] = c["opacities"].reshape(-1) if c["opacities"] is not None else None
     losses, images, num_rendered = [], [], []
     radii_max = torch.zeros((P,), dtype=torch.int32, device=dev)
+    cam_chain = {}      # id(camera tensor) -> [tensor, summed gradient]  (bg_color is shared by every view)
+
+    def camera_targets(rss):
+        """{key: zeroed [V, n] float32} for the camera tensors of `rss` that require grad (None when there are none)."""
+        keys = [k for k in _dgr.CAMERA_KEYS if any(getattr(rs, k).requires_grad for rs in rss)]
+        if not keys:
+            return None
+        if grad_chunks > 1 or on_grad_chunk is not None or peers is not None:
+            raise ValueError("render_views_backward: cameras that require grad cannot be combined with grad_chunks > 1, "
+                             "on_grad_chunk or peers (the camera gradient is a sum over all gaussians of one view)")
+        return {k: torch.zeros((len(rss), _dgr._CAMERA_NUMEL[k]), dtype=torch.float32, device=dev) for k in keys}
+
+    def chain_camera(rss, cam_grads):
+        for k, g in (cam_grads or {}).items():
+            for vi, rs in enumerate(rss):
+                t = getattr(rs, k)
+                if t.requires_grad:
+                    entry = cam_chain.setdefault(id(t), [t, torch.zeros_like(t)])
+                    entry[1] += g[vi].view(t.shape).to(t.dtype)
+
     cams_all = list(viewpoint_cameras) if batched else None
     if batched and cams_all and all(int(cm.image_height) == int(cams_all[0].image_height) and
                                     int(cm.image_width) == int(cams_all[0].image_width) for cm in cams_all):
@@ -278,10 +303,12 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
             if densify_stats is not None:
                 vg["means2D"] = torch.empty((len(chunk), P, 3), dtype=torch.float32, device=dev)
             last_chunk = c0 + _dgr.MAX_BATCH_VIEWS >= len(cams_all)     # gradients are final only after the last view chunk
+            cam_grads = camera_targets(rss)
             _dgr._backward_batch_impl(pack, rss, c["means3D"], c["shs"], c["opacities"], c["scales"], c["rotations"], color,
                                       invdepth, g_color, g_depth, vg, accumulate=not (overwrite and c0 == 0),
                                       n_chunks=grad_chunks if last_chunk else 1, on_chunk=on_grad_chunk if last_chunk else None,
-                                      peers=peers)
+                                      peers=peers, cam_grads=cam_grads)
+            chain_camera(rss, cam_grads)
             torch.maximum(radii_max, radii.max(dim=0).values, out=radii_max)
             if densify_stats is not None:
                 vis = radii > 0                                               # [V,P]
@@ -308,9 +335,12 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         vg = dict(grads)
         if densify_stats is not None:
             vg["means2D"] = m2d
+        cam_grads = camera_targets([rs])
         _dgr._backward_impl(pack, rs, c["means3D"], c["shs"], None, c["opacities"], c["scales"], c["rotations"], None,
                             color.detach(), invdepth.detach(), _dgr._f32c(g_img), _dgr._f32c(g_dep), vg,
-                            accumulate=not (overwrite and vi == 0), accumulate_means2D=False)
+                            accumulate=not (overwrite and vi == 0), accumulate_means2D=False,
+                            cam_grads={k: g[0] for k, g in cam_grads.items()} if cam_grads else None)
+        chain_camera([rs], cam_grads)
         torch.maximum(radii_max, radii, out=radii_max)
         if densify_stats is not None:
             # add_densification_stats (gaussian_model.py:471-473) + max_radii2D update (train.py:166), sync-free
@@ -327,6 +357,9 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         if not direct and v.requires_grad:
             chain_t.append(v)
             chain_g.append(g.view_as(v))
+    for t, g in cam_chain.values():
+        chain_t.append(t)
+        chain_g.append(g)
     if chain_t:
         torch.autograd.backward(chain_t, chain_g)
     if hasattr(pc, "gradients_ready"):      # gaussian_store.GaussianModel: its gradient buffer now belongs to the current parameters

@@ -165,6 +165,31 @@ int32_t gsb_backward_split_sh(const GsbSettings *settings, const GsbInputs *in, 
                               const float *dL_dinvdepth, const GsbGrads *grads, int32_t accumulate,
                               gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
 
+/* Camera gradients: gsb_backward (split == NULL) or gsb_backward_split_sh that also returns dL/d of the camera tensors of
+ * `settings` (a learnable pose, a learnable background).  Every output is optional; with cam_grads NULL or all four fields
+ * NULL the call is gsb_backward / gsb_backward_split_sh.  Outputs have the layout of the matching settings input (viewmatrix /
+ * projmatrix: transposed, row-major, [r][c] at 4r+c) and are written (accumulate != 0: added to).  Conventions:
+ *  - the gradient is that of the forward as computed: the 1.3x frustum clamp of x/z, y/z is a constant (no gradient through
+ *    a clamped coordinate), the SH clamp to 0 and the anti-aliasing factor act as in dL/dmeans3D, and a gaussian that no
+ *    pixel blended contributes nothing;
+ *  - column 3 of the viewmatrix and column 2 of the projmatrix are never read by the forward: their gradient is 0;
+ *  - dL/dcampos is 0 with colors_precomp (campos only enters through the SH view direction);
+ *  - dL/dbg[c] = sum over pixels of final transmittance * dL/dcolor[c].
+ * The per-gaussian terms are summed per warp inside the backward preprocess kernel and then over the warps by one small kernel
+ * in a fixed order (no float atomics): repeated calls give identical bits.  No host synchronisation.
+ * Not available on gsb_backward_batch_chunked / gsb_backward_batch_peer: the per-view sum would have to span the gaussian
+ * chunks (which the caller consumes while later chunks run) or the ranks. */
+typedef struct GsbCameraGrads {
+    float *dL_dviewmatrix;  /* [16] (batch: [V,16]) or NULL, layout of the viewmatrix input */
+    float *dL_dprojmatrix;  /* [16] (batch: [V,16]) or NULL */
+    float *dL_dcampos;      /* [3]  (batch: [V,3])  or NULL */
+    float *dL_dbg;          /* [3]  (batch: [V,3])  or NULL */
+} GsbCameraGrads;
+int32_t gsb_backward_camera(const GsbSettings *settings, const GsbInputs *in, const GsbSplitSH *split /* NULL = joint shs */,
+                            const GsbState *state, const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                            const float *dL_dinvdepth, const GsbGrads *grads, const GsbCameraGrads *cam_grads, int32_t accumulate,
+                            gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
+
 /* View-batch variants (DESIGN.md section 5): V <= 16 cameras of equal image size against the SAME gaussians.
  * The per-gaussian parameters are read once for all views (preprocess), the V depth sorts / scans / tile sorts
  * run as single batched launches, and there is ONE host read-back (V instance counts) per call.
@@ -178,6 +203,11 @@ int32_t gsb_backward_batch(int32_t V, const GsbSettings *settings, const GsbInpu
                            const float *out_color, const float *out_invdepth, const float *dL_dcolor,
                            const float *dL_dinvdepth, const GsbGrads *grads, int32_t accumulate,
                            gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
+/* gsb_backward_batch that also returns each view's camera gradient (GsbCameraGrads; outputs [V,16] / [V,3], one row per view). */
+int32_t gsb_backward_batch_camera(int32_t V, const GsbSettings *settings, const GsbInputs *in, const GsbState *states,
+                                  const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                                  const float *dL_dinvdepth, const GsbGrads *grads, const GsbCameraGrads *cam_grads,
+                                  int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
 
 /* gsb_forward_batch without ANY host synchronisation (what lets the host enqueue whole training steps ahead of the
  * device, and what a CUDA-graph capture of the step needs).  `capacity` (> 0) is the per-view instance capacity of the
