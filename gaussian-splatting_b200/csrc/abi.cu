@@ -408,11 +408,12 @@ static void set_cam_outputs(const GsbCameraGrads *cg, CamReduceArgs &r) {
     r.dview = cg->dL_dviewmatrix; r.dproj = cg->dL_dprojmatrix; r.dcampos = cg->dL_dcampos; r.dbg = cg->dL_dbg;
 }
 
-// shared body of gsb_backward (split == NULL), gsb_backward_split_sh and gsb_backward_camera (cam_grads != NULL)
+// shared body of gsb_backward (split == NULL), gsb_backward_split_sh, gsb_backward_camera (cam_grads != NULL) and
+// gsb_backward_alpha (dL_dalpha != NULL)
 static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
                          const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
                          const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream,
-                         const GsbCameraGrads *cam_grads = nullptr) {
+                         const GsbCameraGrads *cam_grads = nullptr, const float *dL_dalpha = nullptr) {
     if (!s || !in || !st || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc) {
         set_error("%s: NULL argument", fn);
         return GSB_ERR_ARGUMENT;
@@ -458,6 +459,7 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
         ra.tile_order = static_cast<const uint32_t *>(st->tile_order);
         ra.splat = splat; ra.n_contrib = st->n_contrib; ra.dL_dcolor = dL_dcolor;
         ra.dL_dinvdepth = dL_dinvdepth; ra.dacc = dacc; ra.out_color = out_color; ra.out_invdepth = out_invdepth;
+        ra.final_T = st->final_T; ra.dL_dalpha = dL_dalpha;
         rc = launch_render_bwd(ra, debug, stream);
         if (rc) return rc;
     }
@@ -498,6 +500,38 @@ int32_t gsb_backward_camera(const GsbSettings *s, const GsbInputs *in, const Gsb
                             void *alloc_ctx, void *cuda_stream) {
     return backward_impl("gsb_backward_camera", s, in, split, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate,
                          alloc, alloc_ctx, cuda_stream, cam_grads);
+}
+
+int32_t gsb_backward_alpha(const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
+                           const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
+                           const float *dL_dalpha, const GsbGrads *grads, const GsbCameraGrads *cam_grads, int32_t accumulate,
+                           gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {
+    if (dL_dalpha && (reinterpret_cast<size_t>(dL_dalpha) & 3)) {
+        set_error("gsb_backward_alpha: dL_dalpha must be a 4-byte aligned float pointer");
+        return GSB_ERR_ARGUMENT;
+    }
+    return backward_impl("gsb_backward_alpha", s, in, split, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate,
+                         alloc, alloc_ctx, cuda_stream, cam_grads, dL_dalpha);
+}
+
+int32_t gsb_alpha(int32_t V, const GsbState *states, int32_t height, int32_t width, float *out_alpha, void *cuda_stream) {
+    if (!states || !out_alpha || V < 1 || V > GSB_MAX_VIEWS || height <= 0 || width <= 0) {
+        set_error("gsb_alpha: NULL argument, V=%d outside 1..%d or bad image size %d x %d", V, GSB_MAX_VIEWS, height, width);
+        return GSB_ERR_ARGUMENT;
+    }
+    AlphaArgs a;
+    memset(&a, 0, sizeof(a));
+    a.V = V; a.npix = (size_t)height * width; a.out = out_alpha;
+    for (int v = 0; v < V; ++v) {
+        // the IMAGE buffer holds final_T and n_contrib of npix pixels each (carve_image): a smaller one is another image size
+        if (!states[v].final_T || !states[v].image ||
+            (const char *)states[v].final_T + a.npix * sizeof(float) > (const char *)states[v].image + states[v].image_bytes) {
+            set_error("gsb_alpha: state %d has no forward image of %d x %d pixels", v, width, height);
+            return GSB_ERR_ARGUMENT;
+        }
+        a.final_T[v] = states[v].final_T;
+    }
+    return launch_alpha(a, false, static_cast<cudaStream_t>(cuda_stream));
 }
 
 static int check_batch(int32_t V, const GsbSettings *s, const GsbInputs *in, CamArgsBatch &cb) {
@@ -714,7 +748,7 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
                                const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth, const GsbGrads *grads,
                                int32_t accumulate, int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx, gsb_alloc_fn alloc,
                                void *alloc_ctx, cudaStream_t stream, const GsbPeerTable *peers = nullptr,
-                               const GsbCameraGrads *cam_grads = nullptr) {
+                               const GsbCameraGrads *cam_grads = nullptr, const float *dL_dalpha = nullptr) {
     CamArgsBatch cb;
     int rc = check_batch(V, s, in, cb);
     if (rc) return rc;
@@ -757,6 +791,7 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
         ra.tile_order = static_cast<const uint32_t *>(states[0].tile_order);
         ra.splat = static_cast<const float4 *>(states[0].splat); ra.n_contrib = states[0].n_contrib;
         ra.dL_dcolor = dL_dcolor; ra.dL_dinvdepth = dL_dinvdepth; ra.dacc = dacc; ra.out_color = out_color; ra.out_invdepth = out_invdepth;
+        ra.final_T = states[0].final_T; ra.dL_dalpha = dL_dalpha;     // final_T and n_contrib share the IMAGE stride sv_image
         rc = launch_render_bwd(ra, debug, stream);
         if (rc) return rc;
     }
@@ -850,6 +885,26 @@ int32_t gsb_backward_batch_chunked(int32_t V, const GsbSettings *s, const GsbInp
     }
     return backward_batch_impl(V, s, in, states, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate, n_chunks, on_chunk,
                                chunk_ctx, alloc, alloc_ctx, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int32_t gsb_backward_batch_alpha(int32_t V, const GsbSettings *s, const GsbInputs *in, const GsbState *states, const float *out_color,
+                                 const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth, const float *dL_dalpha,
+                                 const GsbGrads *grads, const GsbCameraGrads *cam_grads, const GsbPeerTable *peers, int32_t accumulate,
+                                 int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx, gsb_alloc_fn alloc, void *alloc_ctx,
+                                 void *cuda_stream) {
+    if (!s || !in || !states || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc || in->P <= 0 || n_chunks < 1 ||
+        n_chunks > 64) {
+        set_error("gsb_backward_batch_alpha: NULL argument, empty input or n_chunks outside 1..64");
+        return GSB_ERR_ARGUMENT;
+    }
+    if (dL_dalpha && (reinterpret_cast<size_t>(dL_dalpha) & 3)) {
+        set_error("gsb_backward_batch_alpha: dL_dalpha must be a 4-byte aligned float pointer");
+        return GSB_ERR_ARGUMENT;
+    }
+    // the existing entry points' mode selection: peers take the peer path (always adding), else chunks, else plain
+    if (peers) { accumulate = 1; n_chunks = 1; on_chunk = nullptr; }
+    return backward_batch_impl(V, s, in, states, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate, n_chunks, on_chunk,
+                               chunk_ctx, alloc, alloc_ctx, static_cast<cudaStream_t>(cuda_stream), peers, cam_grads, dL_dalpha);
 }
 
 // ---- peer memory (one process per GPU of a node): allocation + CUDA IPC, for the fused reduce-scatter ----

@@ -117,6 +117,17 @@ struct RenderBwdArgs {
     const float *out_color, *out_invdepth;   // forward outputs
     const float *dL_dcolor, *dL_dinvdepth;
     float *dacc;
+    // rendered-alpha gradient (alpha = 1 - final_T): dL_dalpha [V][H*W] at stride sv_depth, final_T at stride sv_image; NULL =
+    // no alpha term.  Appended last so that the parameter offsets of the kernels that do not read them stay where they were.
+    const float *final_T, *dL_dalpha;
+};
+
+// alpha[v][p] = 1 - final_T[v][p] for V <= GSB_MAX_VIEWS forward states (any mix of single-view and view-batch calls)
+struct AlphaArgs {
+    int V;
+    size_t npix;
+    const float *final_T[GSB_MAX_VIEWS];
+    float *out;           // [V][npix]
 };
 
 // split: a.shs / a.rest are the split SH input (see PreFwdArgs)
@@ -139,6 +150,7 @@ int launch_tile_ranges(const uint32_t *sorted_tiles, int64_t D, const unsigned l
 
 int launch_render_fwd(const RenderFwdArgs &a, bool debug, cudaStream_t stream);
 int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream);
+int launch_alpha(const AlphaArgs &a, bool debug, cudaStream_t stream);
 int launch_tile_order(const uint2 *ranges, int V, int num_tiles, uint32_t *order, bool debug, cudaStream_t stream);
 int launch_l1_loss_grad(const float *img, const float *gt, int64_t n, float scale, float *grad, float *loss_accum,
                         cudaStream_t stream);

@@ -31,6 +31,8 @@
 namespace gsb {
 
 constexpr int RB = 256;  // gaussians staged per round, forward
+// CTAs per SM the backward kernels with the alpha channel are compiled for (no spills on sm_90a; DESIGN.md section 7.6)
+constexpr int ALPHA_MINB = 14, ALPHA_DEPTH_MINB = 12;
 
 // One staged gaussian = ONE 48-byte shared-memory record, so that the blend loops form one address per list entry and read the
 // record with two or three 128-bit loads at fixed offsets.  (Separate arrays meant one address computation each, the third one --
@@ -177,7 +179,10 @@ __device__ __forceinline__ void red_add_if(char *base, const int off, const floa
 }
 
 // Backward.  Arithmetic per lane is IEEE round-to-nearest (the f32x2 helpers are pairs of _rn scalar instructions).
-template <bool DEPTH, int MINB>
+// ALPHA: the rendered alpha A = 1 - final_T is one more channel whose per-gaussian "colour" is 1 and whose background is 0:
+// g_k += dL/dA and S += dL/dA * A.  Then T_k - (A - F_k) / (1 - alpha_k) = T_final / (1 - alpha_k) = dA/dalpha_k, as it must.
+// It has no colour gradient, so the accumulator row, the shuffle networks and the reduction are those of the plain kernel.
+template <bool DEPTH, bool ALPHA, int MINB>
 __global__ void __launch_bounds__(64, MINB)
 render_bwd_kernel(const RenderBwdArgs a) {
     constexpr int NT = 64;
@@ -205,12 +210,12 @@ render_bwd_kernel(const RenderBwdArgs a) {
     const size_t HW = (size_t)a.W * a.H;
 
     // per-pixel state, packed by row: element c of row r is pixel (px0 + c, py0 + r)
-    f32x2 T[2], F[2], S[2], dL0[2], dL1[2], dL2[2], dLd[2];
+    f32x2 T[2], F[2], S[2], dL0[2], dL1[2], dL2[2], dLd[2], dLa[2];
     uint32_t last[4];
     uint32_t my_max = 0;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-        float vS[2] = {0.f, 0.f}, v0[2] = {0.f, 0.f}, v1[2] = {0.f, 0.f}, v2[2] = {0.f, 0.f}, vd[2] = {0.f, 0.f};
+        float vS[2] = {0.f, 0.f}, v0[2] = {0.f, 0.f}, v1[2] = {0.f, 0.f}, v2[2] = {0.f, 0.f}, vd[2] = {0.f, 0.f}, va[2] = {0.f, 0.f};
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
             const int px = px0 + c, py = py0 + r;
@@ -221,11 +226,13 @@ render_bwd_kernel(const RenderBwdArgs a) {
                 v0[c] = dL_dcolor[pid]; v1[c] = dL_dcolor[HW + pid]; v2[c] = dL_dcolor[2 * HW + pid];
                 vS[c] = v0[c] * out_color[pid] + v1[c] * out_color[HW + pid] + v2[c] * out_color[2 * HW + pid];
                 if (DEPTH) { vd[c] = a.dL_dinvdepth[v * a.sv_depth + pid]; vS[c] += vd[c] * a.out_invdepth[v * a.sv_depth + pid]; }
+                if (ALPHA) { va[c] = a.dL_dalpha[v * a.sv_depth + pid]; vS[c] += va[c] * (1.0f - a.final_T[v * a.sv_image + pid]); }
             }
             my_max = max(my_max, last[2 * r + c]);
         }
         T[r] = pk1(1.0f); F[r] = pk1(0.0f); S[r] = pk(vS[0], vS[1]);
         dL0[r] = pk(v0[0], v0[1]); dL1[r] = pk(v1[0], v1[1]); dL2[r] = pk(v2[0], v2[1]); dLd[r] = pk(vd[0], vd[1]);
+        dLa[r] = pk(va[0], va[1]);
     }
     if (t == 0) s_max = 0;
     __syncthreads();
@@ -303,6 +310,7 @@ render_bwd_kernel(const RenderBwdArgs a) {
                 const f32x2 w = mul2(ai, T[r]);
                 f32x2 g = fma2(dL2[r], cb, fma2(dL1[r], cg, mul2(dL0[r], cr)));
                 if (DEPTH) g = fma2(dLd[r], cd, g);
+                if (ALPHA) g = add2(g, dLa[r]);
                 F[r] = fma2(w, g, F[r]);
                 if (r == 0) {
                     g_r = mul2(w, dL0[r]); g_g = mul2(w, dL1[r]); g_b = mul2(w, dL2[r]);
@@ -414,11 +422,45 @@ int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream) {
     if (tiles <= 0) return GSB_OK;
     int rc = check_views("render_bwd", a.V, tiles);
     if (rc) return rc;
-    if (a.dL_dinvdepth) {
-        GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<true, 12>), dim3(tiles, a.V), 64, 0, a);
-    } else {   // register budget for 16 CTAs/SM (64 registers, no spills on sm_90a)
-        GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<false, 16>), dim3(tiles, a.V), 64, 0, a);
+    if (a.dL_dalpha && !a.final_T) {
+        set_error("render_bwd: dL_dalpha without final_T");
+        return GSB_ERR_ARGUMENT;
     }
+    if (a.dL_dalpha) {   // register budgets: DESIGN.md section 7.6
+        if (a.dL_dinvdepth) {
+            GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<true, true, ALPHA_DEPTH_MINB>), dim3(tiles, a.V), 64, 0, a);
+        } else {
+            GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<false, true, ALPHA_MINB>), dim3(tiles, a.V), 64, 0, a);
+        }
+    } else if (a.dL_dinvdepth) {
+        GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<true, false, 12>), dim3(tiles, a.V), 64, 0, a);
+    } else {   // register budget for 16 CTAs/SM (64 registers, no spills on sm_90a)
+        GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<false, false, 16>), dim3(tiles, a.V), 64, 0, a);
+    }
+    return GSB_OK;
+}
+
+// Rendered alpha of V forward states: one launch, blockIdx.y = view.  The forward leaves final_T in every state's IMAGE buffer;
+// nothing else is read.
+__global__ void __launch_bounds__(256)
+alpha_kernel(const AlphaArgs a) {
+    const float *T = a.final_T[0];
+#pragma unroll
+    for (int k = 1; k < GSB_MAX_VIEWS; ++k)
+        if (k == (int)blockIdx.y) T = a.final_T[k];
+    float *out = a.out + (size_t)blockIdx.y * a.npix;
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < a.npix; i += (size_t)gridDim.x * 256)
+        out[i] = __fsub_rn(1.0f, __ldg(T + i));
+}
+
+int launch_alpha(const AlphaArgs &a, bool debug, cudaStream_t stream) {
+    if (a.npix == 0) return GSB_OK;
+    if (a.V < 1 || a.V > GSB_MAX_VIEWS) {
+        set_error("alpha: bad launch geometry (V=%d)", a.V);
+        return GSB_ERR_ARGUMENT;
+    }
+    const size_t blocks = (a.npix + 255) / 256;
+    GSB_LAUNCH("render_alpha", debug, stream, alpha_kernel, dim3((unsigned)(blocks < 4096 ? blocks : 4096), a.V), 256, 0, a);
     return GSB_OK;
 }
 

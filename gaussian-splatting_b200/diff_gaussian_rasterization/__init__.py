@@ -127,6 +127,17 @@ def _load(path: Optional[str] = None):
     lib.gsb_backward_batch_camera.argtypes = [c_int32, POINTER(_Settings), POINTER(_Inputs), POINTER(_State), c_void_p, c_void_p,
                                               c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads), c_int32, _ALLOC_FN,
                                               c_void_p, c_void_p]
+    lib.gsb_alpha.restype = c_int32
+    lib.gsb_alpha.argtypes = [c_int32, POINTER(_State), c_int32, c_int32, c_void_p, c_void_p]
+    lib.gsb_backward_alpha.restype = c_int32
+    lib.gsb_backward_alpha.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), POINTER(_State), c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads), c_int32, _ALLOC_FN,
+                                       c_void_p, c_void_p]
+    lib.gsb_backward_batch_alpha.restype = c_int32
+    lib.gsb_backward_batch_alpha.argtypes = [c_int32, POINTER(_Settings), POINTER(_Inputs), POINTER(_State), c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads),
+                                             POINTER(_PeerTable), c_int32, c_int32, _CHUNK_FN, c_void_p, _ALLOC_FN, c_void_p,
+                                             c_void_p]
     lib.gsb_sparse_adam_step.restype = c_int32
     lib.gsb_sparse_adam_step.argtypes = [POINTER(_SparseAdamGroup), c_int32, c_void_p, c_int64, c_float, c_float, c_void_p]
     lib.gsb_forward_batch.restype = c_int32
@@ -579,6 +590,18 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
     return color, radii, invdepth, pack
 
 
+def _alpha_impl(states, height: int, width: int, device) -> torch.Tensor:
+    """Rendered alpha (1 - final transmittance, gsb_alpha) of the forward states ``states`` (a ``_State`` or a ctypes array of
+    them, e.g. a pack's "state" / "states"): [V,1,H,W] for an array, [1,H,W] for one state.  One launch, no synchronisation."""
+    one = isinstance(states, _State)
+    V = 1 if one else len(states)
+    out = torch.empty((V, 1, int(height), int(width)), dtype=torch.float32, device=device)
+    with _device_ctx(device):
+        rc = _C.gsb_alpha(V, byref(states) if one else states, int(height), int(width), out.data_ptr(), _current_stream(device))
+    _check(rc)
+    return out[0] if one else out
+
+
 CAMERA_KEYS = ("viewmatrix", "projmatrix", "campos", "bg")     # GsbCameraGrads, in field order
 _CAMERA_NUMEL = dict(viewmatrix=16, projmatrix=16, campos=3, bg=3)
 
@@ -603,12 +626,14 @@ def _camera_grads(cam_grads: Optional[dict], V: Optional[int] = None):
 
 def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                    out_color, out_invdepth, grad_color, grad_invdepth, grads: dict, accumulate: bool,
-                   accumulate_means2D: Optional[bool] = None, dc=None, cam_grads: Optional[dict] = None):
+                   accumulate_means2D: Optional[bool] = None, dc=None, cam_grads: Optional[dict] = None,
+                   grad_alpha: Optional[torch.Tensor] = None):
     """grads: tensors to fill (accumulate=False) or add into (accumulate=True).  The C ABI has one accumulate
     switch; a per-view means2D buffer (accumulate_means2D=False while the rest accumulates) is zeroed here.
     ``dc``: split SH input (gsb_backward_split_sh); ``sh`` is the rest, grads["dc"] / grads["shs"] receive their gradients.
     ``cam_grads``: {"viewmatrix": [16], "projmatrix": [16], "campos": [3], "bg": [3]} float32 tensors (any subset) that receive
-    the camera gradient under the same accumulate switch (gsb_backward_camera)."""
+    the camera gradient under the same accumulate switch (gsb_backward_camera).  ``grad_alpha``: dL/d rendered alpha [1,H,W]
+    float32 contiguous, or None (gsb_backward_alpha; None takes the calls above)."""
     if accumulate and accumulate_means2D is False and grads.get("means2D") is not None:
         grads["means2D"].zero_()
     dev = means3D.device
@@ -626,7 +651,13 @@ def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rot
         stream = _current_stream(dev)
         arena = _Arena(dev, stream)
         cg = _camera_grads(cam_grads)
-        if cg is not None:
+        if grad_alpha is not None:
+            sp = _split_sh(dc, sh, grads) if dc is not None else None
+            rc = _C.gsb_backward_alpha(byref(cs), byref(ci), byref(sp) if sp is not None else None, byref(pack["state"]),
+                                       out_color.data_ptr(), out_invdepth.data_ptr(), grad_color.data_ptr(), _ptr(grad_invdepth),
+                                       grad_alpha.data_ptr(), byref(g), byref(cg) if cg is not None else None,
+                                       int(bool(accumulate)), arena.cb, None, stream)
+        elif cg is not None:
             sp = _split_sh(dc, sh, grads) if dc is not None else None
             rc = _C.gsb_backward_camera(byref(cs), byref(ci), byref(sp) if sp is not None else None, byref(pack["state"]),
                                         out_color.data_ptr(), out_invdepth.data_ptr(), grad_color.data_ptr(), _ptr(grad_invdepth),
@@ -695,7 +726,7 @@ def capacity_for(count: int) -> int:
 
 def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, rotations, out_color, out_invdepth,
                          grad_color, grad_invdepth, grads: dict, accumulate: bool, n_chunks: int = 1, on_chunk=None, peers=None,
-                         cam_grads: Optional[dict] = None):
+                         cam_grads: Optional[dict] = None, grad_alpha: Optional[torch.Tensor] = None):
     """View-batch backward (gsb_backward_batch).  grads: tensors holding / receiving the gradient SUMMED over the views
     (means2D, if present, is [V,P,3] and per view).  ``n_chunks`` > 1: gsb_backward_batch_chunked -- the last kernel runs in
     gaussian-range chunks and ``on_chunk(chunk, p_begin, p_end)`` is called after each chunk has been enqueued (rows
@@ -703,7 +734,8 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
     [base pointers]): gsb_backward_batch_peer -- the gradients are ADDED into the owner ranks' buffers (fused reduce-scatter;
     gaussian_renderer.peer.PeerGradientBucket drives the protocol around it).  ``cam_grads``: {"viewmatrix": [V,16],
     "projmatrix": [V,16], "campos": [V,3], "bg": [V,3]} float32 tensors (any subset) receiving each view's camera gradient
-    (gsb_backward_batch_camera); not with ``n_chunks`` > 1, ``on_chunk`` or ``peers``."""
+    (gsb_backward_batch_camera); not with ``n_chunks`` > 1, ``on_chunk`` or ``peers``.  ``grad_alpha``: dL/d rendered alpha
+    [V,1,H,W] float32 contiguous, or None; with it every mode goes through gsb_backward_batch_alpha."""
     dev = means3D.device
     V, P = pack["V"], int(means3D.shape[0])
     cg = _camera_grads(cam_grads, V)
@@ -720,23 +752,35 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
         g.dL_dscales, g.dL_drotations = _ptr(grads.get("scales")), _ptr(grads.get("rotations"))
         stream = _current_stream(dev)
         arena = _Arena(dev, stream)
+        pt = None
         if peers is not None:
             world, rank, rows_per_rank, bases = peers
             pt = _PeerTable()
             pt.world, pt.rank, pt.rows_per_rank, pt.reserved = int(world), int(rank), int(rows_per_rank), 0
             pt.base = (c_void_p * 16)(*([int(b) for b in bases] + [None] * (16 - len(bases))))
+        err = []
+
+        def _cb(_ctx, chunk, p0, p1):
+            try:
+                if on_chunk is not None and not err:
+                    on_chunk(int(chunk), int(p0), int(p1))
+            except Exception as e:  # never let an exception cross the C ABI
+                err.append(e)
+        if grad_alpha is not None:
+            chunked = pt is None and (n_chunks > 1 or on_chunk is not None)
+            cb = _CHUNK_FN(_cb) if chunked else _CHUNK_FN()     # NULL callback
+            rc = _C.gsb_backward_batch_alpha(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
+                                             grad_color.data_ptr(), _ptr(grad_invdepth), grad_alpha.data_ptr(), byref(g),
+                                             byref(cg) if cg is not None else None, byref(pt) if pt is not None else None,
+                                             int(bool(accumulate)), int(n_chunks) if chunked else 1, cb, None, arena.cb, None, stream)
+            _check(rc, arena)
+            if err:
+                raise err[0]
+        elif pt is not None:
             rc = _C.gsb_backward_batch_peer(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
                                             grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), byref(pt), arena.cb, None, stream)
             _check(rc, arena)
         elif n_chunks > 1 or on_chunk is not None:
-            err = []
-
-            def _cb(_ctx, chunk, p0, p1):
-                try:
-                    if on_chunk is not None and not err:
-                        on_chunk(int(chunk), int(p0), int(p1))
-                except Exception as e:  # never let an exception cross the C ABI
-                    err.append(e)
             cb = _CHUNK_FN(_cb)
             rc = _C.gsb_backward_batch_chunked(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
                                                grad_color.data_ptr(), _ptr(grad_invdepth), byref(g), int(bool(accumulate)),
@@ -757,15 +801,19 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, dc=None):
+                        raster_settings, dc=None, return_alpha=False):
     """``dc`` (optional): split SH input -- ``dc`` [P,1,3] holds the DC coefficient and ``sh`` [P,M-1,3] the others (M-1 may
     be 0); the result equals that of ``sh = cat((dc, sh), 1)`` without the concatenation.
 
     Camera gradients: when grad mode is on and any of ``raster_settings.viewmatrix`` / ``.projmatrix`` / ``.campos`` / ``.bg``
     requires grad, the four tensors become trailing inputs of the autograd function and those that require grad receive
-    their gradient (gsb_backward_camera; conventions in include/gs_b200.h).  Otherwise the call is exactly the plain one."""
+    their gradient (gsb_backward_camera; conventions in include/gs_b200.h).  Otherwise the call is exactly the plain one.
+
+    ``return_alpha=True``: the result is (color, radii, invdepth, alpha[1,H,W]) with alpha = 1 - final transmittance (gsb_alpha;
+    definition in include/gs_b200.h), differentiable w.r.t. every gaussian input and the camera tensors.  One extra launch in the
+    forward; a backward in which alpha's gradient is unused (None) is the plain one."""
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings, dc, *_camera_inputs(raster_settings))
+                                     cov3Ds_precomp, raster_settings, dc, bool(return_alpha), *_camera_inputs(raster_settings))
 
 
 def _camera_inputs(rs) -> tuple:
@@ -779,7 +827,7 @@ def _camera_inputs(rs) -> tuple:
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, dc=None, *camera):
+                raster_settings, dc=None, return_alpha=False, *camera):
         # camera: the settings' (viewmatrix, projmatrix, campos, bg) as inputs of their own (rasterize_gaussians), or ()
         args = [_f32c(means3D), _f32c(sh), _f32c(colors_precomp), _f32c(opacities), _f32c(scales), _f32c(rotations),
                 _f32c(cov3Ds_precomp)]
@@ -805,10 +853,13 @@ class _RasterizeGaussians(torch.autograd.Function):
                               dcc if dcc is not None else torch.empty(0))
         ctx.mark_non_differentiable(radii)
         ctx.camera = [(tuple(t.shape), t.dtype) for t in camera]
+        if return_alpha:
+            alpha = _alpha_impl(pack["state"], int(raster_settings.image_height), int(raster_settings.image_width), color.device)
+            return color, radii, invdepth, alpha
         return color, radii, invdepth
 
     @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth):
+    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth, grad_out_alpha=None):
         rs = ctx.raster_settings
         saved = [t if t.numel() > 0 else None for t in ctx.saved_tensors[:7]]
         means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp = saved
@@ -834,23 +885,26 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads["scales"] = new(P, 3)
             grads["rotations"] = new(P, 4)
         cam_grads = {k: torch.empty(_CAMERA_NUMEL[k], dtype=torch.float32, device=dev)
-                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[10 + j]}
-        if grad_out_color is None and grad_out_depth is None:
-            return (None,) * (10 + len(ctx.camera))
+                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[11 + j]}
+        if grad_out_color is None and grad_out_depth is None and grad_out_alpha is None:
+            return (None,) * (11 + len(ctx.camera))
         gc = _f32c(grad_out_color)
         if gc is None:
             gc = torch.zeros((3, int(rs.image_height), int(rs.image_width)), dtype=torch.float32, device=dev)
         gd = _f32c(grad_out_depth)
+        ga = _f32c(grad_out_alpha)
         if dc is None and "dc" in grads:                         # P == 0
             grads["dc"].zero_()
         try:
             _backward_impl(ctx.pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc, cam_grads=cam_grads)
+                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc, cam_grads=cam_grads, grad_alpha=ga)
         except Exception:
             if rs.debug:
                 split = [ctx.saved_tensors[9].cpu()] if ctx.shapes["dc"] is not None else []
                 camera = [getattr(rs, k).detach().cpu() for k in CAMERA_KEYS] if ctx.camera else []
-                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()] + camera, "snapshot_bw.dump")
+                alpha = [ga.cpu()] if ga is not None else []
+                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()] + camera + alpha,
+                           "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
             raise
         g_op = grads["opacities"].reshape(ctx.shapes["opacities"])
@@ -858,7 +912,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                       for k, (shape, dtype) in zip(CAMERA_KEYS, ctx.camera))
         return (grads["means3D"], grads["means2D"] if ctx.shapes["means2D"] is not None else None, grads.get("shs"),
                 grads.get("colors_precomp"), g_op, grads.get("scales"), grads.get("rotations"),
-                grads.get("cov3D_precomp"), None, grads.get("dc")) + g_cam
+                grads.get("cov3D_precomp"), None, grads.get("dc"), None) + g_cam
 
 
 class GaussianRasterizer(nn.Module):
@@ -882,9 +936,10 @@ class GaussianRasterizer(nn.Module):
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, dc=None):
+                cov3D_precomp=None, dc=None, return_alpha=False):
         """``dc``: the split SH input of the accel branch (gaussian_renderer/__init__.py:90-100) -- ``dc`` [P,1,3] is the DC
-        coefficient and ``shs`` [P,M-1,3] the others (may have zero coefficients); gradients come back in the same split."""
+        coefficient and ``shs`` [P,M-1,3] the others (may have zero coefficients); gradients come back in the same split.
+        ``return_alpha=True``: also returns the rendered alpha [1,H,W] (rasterize_gaussians)."""
         rs = self.raster_settings
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
@@ -894,7 +949,7 @@ class GaussianRasterizer(nn.Module):
         if dc is not None and colors_precomp is not None:
             raise Exception("dc is the SH DC coefficient: it goes with shs, not with precomputed colors!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   rs, dc)
+                                   rs, dc, return_alpha)
 
 
 # SparseGaussianAdam: bound here only on request (module docstring); sparse_adam.py is importable either way

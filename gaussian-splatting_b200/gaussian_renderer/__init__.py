@@ -48,9 +48,10 @@ def _eval_sh(deg, sh, dirs):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, separate_sh=False,
-           override_color=None, use_trained_exp=False):
+           override_color=None, use_trained_exp=False, return_alpha=False):
     """Same contract as the reference's render(): returns
-    {"render", "viewspace_points", "visibility_filter", "radii", "depth"}."""
+    {"render", "viewspace_points", "visibility_filter", "radii", "depth"}.  ``return_alpha=True`` adds "alpha": the rendered
+    accumulated opacity [1,H,W] (1 - final transmittance, differentiable; the exposure of ``use_trained_exp`` does not apply)."""
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -88,17 +89,20 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     else:
         colors_precomp = override_color
 
-    rendered_image, radii, depth_image = rasterizer(
-        means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors_precomp, opacities=pc.get_opacity,
-        scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, dc=dc)
+    out = rasterizer(means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors_precomp, opacities=pc.get_opacity,
+                     scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, dc=dc, return_alpha=return_alpha)
+    rendered_image, radii, depth_image = out[:3]
 
     if use_trained_exp:
         exposure = pc.get_exposure_from_name(viewpoint_camera.image_name)
         rendered_image = torch.matmul(rendered_image.permute(1, 2, 0), exposure[:3, :3]).permute(2, 0, 1) \
             + exposure[:3, 3, None, None]
     rendered_image = rendered_image.clamp(0, 1)
-    return {"render": rendered_image, "viewspace_points": screenspace_points,
-            "visibility_filter": (radii > 0).nonzero(), "radii": radii, "depth": depth_image}
+    result = {"render": rendered_image, "viewspace_points": screenspace_points,
+              "visibility_filter": (radii > 0).nonzero(), "radii": radii, "depth": depth_image}
+    if return_alpha:
+        result["alpha"] = out[3]
+    return result
 
 
 def render_views(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch.Tensor, **kw) -> List[dict]:
@@ -184,7 +188,7 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                           scaling_modifier: float = 1.0, densify_stats: Optional[dict] = None,
                           keep_images: bool = False, loss_returns_grad: bool = False, batched: bool = True,
                           overwrite: bool = False, capacity: Optional[AsyncCapacity] = None, grad_chunks: int = 1,
-                          on_grad_chunk=None, peers=None) -> dict:
+                          on_grad_chunk=None, peers=None, with_alpha: bool = False) -> dict:
     """Fused view-batch training step: forward + loss + backward for every camera, with the per-gaussian
     gradients of ALL views summed in place.
 
@@ -213,6 +217,12 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     receives its gradient like a non-leaf gaussian input: each view's camera gradient comes out of the backward kernels
     (gsb_backward_batch_camera / gsb_backward_camera) and is chained into the camera tensors' graphs at the end.  This is
     not available with ``grad_chunks`` > 1, ``on_grad_chunk`` or ``peers`` (ValueError).
+
+    ``with_alpha=True``: ``loss_fn`` also receives the rendered alpha [1,H,W] (1 - final transmittance) as the keyword ``alpha``
+    and may use it: the autograd mode differentiates through it; with ``loss_returns_grad=True`` it may return
+    ``(loss, dL/d image, dL/d invdepth | None, dL/d alpha | None)``.  The alpha gradient goes into the same backward call in every
+    mode (batched or not, sync or async, chunked, peers); a view batch in which no view returns one takes the plain backward.
+    ``keep_images=True`` also returns "alphas".
     """
     takes_grad_out = False
     if loss_returns_grad:
@@ -238,7 +248,7 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         m2d = torch.empty((P, 3), dtype=torch.float32, device=dev)
     c = {k: _dgr._f32c(v.detach()) for k, v in inputs.items()}
     c["opacities"] = c["opacities"].reshape(-1) if c["opacities"] is not None else None
-    losses, images, num_rendered = [], [], []
+    losses, images, alphas, num_rendered = [], [], [], []
     radii_max = torch.zeros((P,), dtype=torch.int32, device=dev)
     cam_chain = {}      # id(camera tensor) -> [tensor, summed gradient]  (bg_color is shared by every view)
 
@@ -274,20 +284,27 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
             if capacity is not None and not use_async:
                 capacity.learn(pack["num_rendered"])
             num_rendered.extend(pack["num_rendered"])
+            alpha = _dgr._alpha_impl(pack["states"], int(color.shape[-2]), int(color.shape[-1]), dev) if with_alpha else None
             g_color = torch.empty_like(color)
-            g_depth = None
+            g_depth = g_alpha = None
             for k in range(len(chunk)):
                 vi = c0 + k
+                akw = dict(alpha=alpha[k]) if with_alpha else {}
+                g_al = None
                 if loss_returns_grad:
-                    res = loss_fn(color[k], invdepth[k], vi, grad_out=g_color[k]) if takes_grad_out else loss_fn(color[k], invdepth[k], vi)
+                    res = loss_fn(color[k], invdepth[k], vi, grad_out=g_color[k], **akw) if takes_grad_out else \
+                        loss_fn(color[k], invdepth[k], vi, **akw)
                     loss, g_img = res[0], res[1]
                     g_dep = res[2] if len(res) > 2 else None
+                    g_al = res[3] if with_alpha and len(res) > 3 else None
                 else:
                     img = color[k].detach().requires_grad_(True)
                     dep = invdepth[k].detach().requires_grad_(True)
+                    akw = {a: t.detach().requires_grad_(True) for a, t in akw.items()}
                     with torch.enable_grad():
-                        loss = loss_fn(img.clamp(0, 1), dep, vi)
-                    g_img, g_dep = torch.autograd.grad(loss, (img, dep), allow_unused=True)
+                        loss = loss_fn(img.clamp(0, 1), dep, vi, **akw)
+                    g_img, g_dep, *g_al = torch.autograd.grad(loss, (img, dep, *akw.values()), allow_unused=True)
+                    g_al = g_al[0] if g_al else None
                 if g_img is None:
                     g_color[k].zero_()
                 elif g_img.data_ptr() != g_color[k].data_ptr():
@@ -296,9 +313,15 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                     if g_depth is None:
                         g_depth = torch.zeros_like(invdepth)
                     g_depth[k].copy_(g_dep)
+                if g_al is not None:
+                    if g_alpha is None:
+                        g_alpha = torch.zeros_like(alpha)
+                    g_alpha[k].copy_(g_al.reshape(alpha[k].shape))
                 losses.append(loss.detach().reshape(()))
                 if keep_images:
                     images.append(color[k].detach())
+                    if with_alpha:
+                        alphas.append(alpha[k])
             vg = dict(grads)
             if densify_stats is not None:
                 vg["means2D"] = torch.empty((len(chunk), P, 3), dtype=torch.float32, device=dev)
@@ -307,7 +330,7 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
             _dgr._backward_batch_impl(pack, rss, c["means3D"], c["shs"], c["opacities"], c["scales"], c["rotations"], color,
                                       invdepth, g_color, g_depth, vg, accumulate=not (overwrite and c0 == 0),
                                       n_chunks=grad_chunks if last_chunk else 1, on_chunk=on_grad_chunk if last_chunk else None,
-                                      peers=peers, cam_grads=cam_grads)
+                                      peers=peers, cam_grads=cam_grads, grad_alpha=g_alpha)
             chain_camera(rss, cam_grads)
             torch.maximum(radii_max, radii.max(dim=0).values, out=radii_max)
             if densify_stats is not None:
@@ -320,16 +343,22 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         color, radii, invdepth, pack = _dgr._forward_impl(c["means3D"], c["shs"], None, c["opacities"], c["scales"],
                                                           c["rotations"], None, rs)
         num_rendered.append(pack["num_rendered"])
+        alpha = _dgr._alpha_impl(pack["state"], int(color.shape[-2]), int(color.shape[-1]), dev) if with_alpha else None
+        akw = dict(alpha=alpha) if with_alpha else {}
+        g_al = None
         if loss_returns_grad:
-            res = loss_fn(color, invdepth, vi)
+            res = loss_fn(color, invdepth, vi, **akw)
             loss, g_img = res[0], res[1]
             g_dep = res[2] if len(res) > 2 else None
+            g_al = res[3] if with_alpha and len(res) > 3 else None
         else:
             img = color.requires_grad_(True)
             dep = invdepth.requires_grad_(True)
+            akw = {a: t.requires_grad_(True) for a, t in akw.items()}
             with torch.enable_grad():
-                loss = loss_fn(img.clamp(0, 1), dep, vi)
-            g_img, g_dep = torch.autograd.grad(loss, (img, dep), allow_unused=True)
+                loss = loss_fn(img.clamp(0, 1), dep, vi, **akw)
+            g_img, g_dep, *g_al = torch.autograd.grad(loss, (img, dep, *akw.values()), allow_unused=True)
+            g_al = g_al[0] if g_al else None
             if g_img is None:
                 g_img = torch.zeros_like(color)
         vg = dict(grads)
@@ -339,7 +368,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         _dgr._backward_impl(pack, rs, c["means3D"], c["shs"], None, c["opacities"], c["scales"], c["rotations"], None,
                             color.detach(), invdepth.detach(), _dgr._f32c(g_img), _dgr._f32c(g_dep), vg,
                             accumulate=not (overwrite and vi == 0), accumulate_means2D=False,
-                            cam_grads={k: g[0] for k, g in cam_grads.items()} if cam_grads else None)
+                            cam_grads={k: g[0] for k, g in cam_grads.items()} if cam_grads else None,
+                            grad_alpha=_dgr._f32c(g_al.reshape(alpha.shape)) if g_al is not None else None)
         chain_camera([rs], cam_grads)
         torch.maximum(radii_max, radii, out=radii_max)
         if densify_stats is not None:
@@ -350,6 +380,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         losses.append(loss.detach().reshape(()).clone() if loss_returns_grad else loss.detach())
         if keep_images:
             images.append(color.detach())
+            if with_alpha:
+                alphas.append(alpha.detach())
     # chain the summed gradient into non-leaf inputs' graphs (one pass, view independent)
     chain_t, chain_g = [], []
     for k, v in inputs.items():
@@ -368,6 +400,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
            "num_rendered": num_rendered}      # per view; -1 on the sync-free path (known to the device only)
     if keep_images:
         out["images"] = images
+        if with_alpha:
+            out["alphas"] = alphas
     return out
 
 

@@ -190,6 +190,29 @@ int32_t gsb_backward_camera(const GsbSettings *settings, const GsbInputs *in, co
                             const float *dL_dinvdepth, const GsbGrads *grads, const GsbCameraGrads *cam_grads, int32_t accumulate,
                             gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
 
+/* Rendered alpha (accumulated opacity), DESIGN.md section 7.6:
+ *     alpha[p] = 1 - final_T[p]
+ * where final_T is the transmittance after the last gaussian pixel p blended, under the forward's rules (the 1/255 cut-off,
+ * the 0.99 cap, the T < 1e-4 stop): the final_T every forward call leaves in its state and uses for the background term, so
+ * color = C_fg + (1 - alpha) * bg holds as computed.  Alpha does not depend on bg (dL/dbg of the camera gradient is unchanged
+ * by an alpha loss); empty or fully culled scenes give alpha = 0 and zero gradients.
+ *
+ * gsb_alpha: out_alpha [V, height*width] from V forward states (states[v] of any forward call: single view, split SH, view
+ * batch, async view batch; height x width must be their image size).  One launch, no host synchronisation.  It reads only the
+ * states' IMAGE buffers, which must still be alive. */
+int32_t gsb_alpha(int32_t V, const GsbState *states, int32_t height, int32_t width, float *out_alpha, void *cuda_stream);
+
+/* Backward with a gradient on the rendered alpha: gsb_backward_camera (split NULL = joint shs; cam_grads NULL = no camera
+ * gradient) plus dL_dalpha [H*W].  With dL_dalpha NULL the call is gsb_backward_camera: the same kernels are launched.  The
+ * alpha term enters the per-gaussian gradients (means, opacity, scales / rotations or cov3D, means2D) and the camera
+ * gradient; it adds nothing to the colour / SH gradients. */
+int32_t gsb_backward_alpha(const GsbSettings *settings, const GsbInputs *in, const GsbSplitSH *split /* NULL = joint shs */,
+                           const GsbState *state, const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                           const float *dL_dinvdepth, const float *dL_dalpha, const GsbGrads *grads,
+                           const GsbCameraGrads *cam_grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx,
+                           void *cuda_stream);
+/* (view batch: gsb_backward_batch_alpha, after gsb_backward_batch_peer below) */
+
 /* View-batch variants (DESIGN.md section 5): V <= 16 cameras of equal image size against the SAME gaussians.
  * The per-gaussian parameters are read once for all views (preprocess), the V depth sorts / scans / tile sorts
  * run as single batched launches, and there is ONE host read-back (V instance counts) per call.
@@ -251,6 +274,20 @@ int32_t gsb_backward_batch_peer(int32_t V, const GsbSettings *settings, const Gs
                                 const float *out_color, const float *out_invdepth, const float *dL_dcolor,
                                 const float *dL_dinvdepth, const GsbGrads *grads, const GsbPeerTable *peers,
                                 gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
+
+/* View-batch backward with a gradient on the rendered alpha (see gsb_alpha), dL_dalpha [V, H*W] or NULL, in every mode of the
+ * view-batch backward:
+ *  - plain (n_chunks 1, on_chunk NULL, peers NULL): gsb_backward_batch, or gsb_backward_batch_camera with cam_grads;
+ *  - n_chunks > 1 (1..64) or on_chunk != NULL: gsb_backward_batch_chunked;
+ *  - peers != NULL: gsb_backward_batch_peer (the outputs are always added into the owners' buffers; accumulate is ignored).
+ * cam_grads is not available with chunks or peers, as for the existing entry points.  With dL_dalpha NULL the call is the
+ * matching existing entry point: the same kernels are launched. */
+int32_t gsb_backward_batch_alpha(int32_t V, const GsbSettings *settings, const GsbInputs *in, const GsbState *states,
+                                 const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                                 const float *dL_dinvdepth, const float *dL_dalpha, const GsbGrads *grads,
+                                 const GsbCameraGrads *cam_grads, const GsbPeerTable *peers, int32_t accumulate,
+                                 int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx, gsb_alloc_fn alloc,
+                                 void *alloc_ctx, void *cuda_stream);
 
 /* Lets kernels launched on the CURRENT device dereference pointers into `peer_device`'s memory (cudaDeviceEnablePeerAccess;
  * already-enabled is not an error).  Needed once per peer before gsb_backward_batch_peer is given peer-mapped buffers. */
