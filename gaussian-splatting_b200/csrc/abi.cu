@@ -408,12 +408,48 @@ static void set_cam_outputs(const GsbCameraGrads *cg, CamReduceArgs &r) {
     r.dview = cg->dL_dviewmatrix; r.dproj = cg->dL_dprojmatrix; r.dcampos = cg->dL_dcampos; r.dbg = cg->dL_dbg;
 }
 
-// shared body of gsb_backward (split == NULL), gsb_backward_split_sh, gsb_backward_camera (cam_grads != NULL) and
-// gsb_backward_alpha (dL_dalpha != NULL)
+static bool misaligned(const void *p) { return (reinterpret_cast<size_t>(p) & 3) != 0; }
+
+// the feature term of a backward call (NULL = none); `launch` = the feature blend pass runs (a feature loss is given)
+static int check_features(const char *fn, const GsbFeatures *ft, int P, bool &launch) {
+    launch = false;
+    if (!ft) return GSB_OK;
+    if (ft->channels < 1 || ft->channels > GSB_MAX_FEATURE_CHANNELS) {
+        set_error("%s: feature channels %d outside 1..%d", fn, ft->channels, GSB_MAX_FEATURE_CHANNELS);
+        return GSB_ERR_ARGUMENT;
+    }
+    if (!ft->features && P > 0 && (ft->out_features || ft->dL_dout_features || ft->dL_dfeatures)) {
+        set_error("%s: feature outputs given without features", fn);
+        return GSB_ERR_ARGUMENT;
+    }
+    if (ft->dL_dout_features && !ft->out_features) {
+        set_error("%s: dL_dout_features given without out_features", fn);
+        return GSB_ERR_ARGUMENT;
+    }
+    if (misaligned(ft->features) || misaligned(ft->out_features) || misaligned(ft->dL_dout_features) || misaligned(ft->dL_dfeatures)) {
+        set_error("%s: feature tensors must be 4-byte aligned float pointers", fn);
+        return GSB_ERR_ARGUMENT;
+    }
+    launch = ft->dL_dout_features != nullptr && P > 0;
+    return GSB_OK;
+}
+
+// a state's view for the feature kernels; false when it does not hold a forward of P gaussians over num_tiles tiles
+static bool feat_view(const GsbState &st, int P, int num_tiles, FeatView &v) {
+    if (st.P != P || st.num_tiles != num_tiles || !st.ranges || !st.point_list || !st.splat || !st.n_contrib) return false;
+    v.ranges = static_cast<const uint2 *>(st.ranges); v.point_list = st.point_list;
+    v.tile_order = static_cast<const uint32_t *>(st.tile_order); v.splat = static_cast<const float4 *>(st.splat);
+    v.n_contrib = st.n_contrib;
+    return true;
+}
+
+// shared body of gsb_backward (split == NULL), gsb_backward_split_sh, gsb_backward_camera (cam_grads != NULL),
+// gsb_backward_alpha (dL_dalpha != NULL) and gsb_backward_features (feat != NULL)
 static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
                          const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
                          const GsbGrads *grads, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream,
-                         const GsbCameraGrads *cam_grads = nullptr, const float *dL_dalpha = nullptr) {
+                         const GsbCameraGrads *cam_grads = nullptr, const float *dL_dalpha = nullptr,
+                         const GsbFeatures *feat = nullptr) {
     if (!s || !in || !st || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc) {
         set_error("%s: NULL argument", fn);
         return GSB_ERR_ARGUMENT;
@@ -437,6 +473,11 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
         set_error("%s: state does not match the inputs (P %d vs %d)", fn, P, st->P);
         return GSB_ERR_ARGUMENT;
     }
+    bool want_feat = false;
+    rc = check_features(fn, feat, P, want_feat);
+    if (rc) return rc;
+    if (feat && feat->dL_dfeatures && !accumulate && P > 0)
+        GSB_CUDA(cudaMemsetAsync(feat->dL_dfeatures, 0, (size_t)P * feat->channels * sizeof(float), stream));
     CamReduceArgs cr;
     memset(&cr, 0, sizeof(cr));
     if (want_cam) {
@@ -462,6 +503,19 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
         ra.final_T = st->final_T; ra.dL_dalpha = dL_dalpha;
         rc = launch_render_bwd(ra, debug, stream);
         if (rc) return rc;
+        if (want_feat) {     // adds its terms into the same accumulator rows (linear in the loss gradient)
+            FeatArgs fa;
+            memset(&fa, 0, sizeof(fa));
+            fa.W = cam.W; fa.H = cam.H; fa.gx = cam.gx; fa.gy = cam.gy; fa.V = 1; fa.C = feat->channels; fa.P = P;
+            if (!feat_view(*st, P, cam.gx * cam.gy, fa.view[0])) {
+                set_error("%s: state has no binning", fn);
+                return GSB_ERR_ARGUMENT;
+            }
+            fa.features = feat->features; fa.out_features = feat->out_features; fa.dL_dout = feat->dL_dout_features;
+            fa.dacc = dacc; fa.dL_dfeatures = feat->dL_dfeatures;
+            rc = launch_render_features_bwd(fa, debug, stream);
+            if (rc) return rc;
+        }
     }
     PreBwdArgs pa;
     pa.P = P; pa.means = in->means3D; pa.shs = split ? split->dc : in->shs; pa.opac = in->opacities; pa.scales = in->scales;
@@ -532,6 +586,49 @@ int32_t gsb_alpha(int32_t V, const GsbState *states, int32_t height, int32_t wid
         a.final_T[v] = states[v].final_T;
     }
     return launch_alpha(a, false, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int32_t gsb_backward_features(const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
+                              const float *out_color, const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth,
+                              const float *dL_dalpha, const GsbGrads *grads, const GsbCameraGrads *cam_grads,
+                              const GsbFeatures *features, int32_t accumulate, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {
+    if (misaligned(dL_dalpha)) {
+        set_error("gsb_backward_features: dL_dalpha must be a 4-byte aligned float pointer");
+        return GSB_ERR_ARGUMENT;
+    }
+    return backward_impl("gsb_backward_features", s, in, split, st, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads,
+                         accumulate, alloc, alloc_ctx, cuda_stream, cam_grads, dL_dalpha, features);
+}
+
+int32_t gsb_render_features(int32_t V, const GsbState *states, int32_t height, int32_t width, int32_t P, int32_t channels,
+                            const float *features, float *out, void *cuda_stream) {
+    if (!states || !out || V < 1 || V > GSB_MAX_VIEWS || height <= 0 || width <= 0 || P < 0 || (P > 0 && !features)) {
+        set_error("gsb_render_features: NULL argument, V=%d outside 1..%d, bad image size %d x %d or P=%d", V, GSB_MAX_VIEWS, height,
+                  width, P);
+        return GSB_ERR_ARGUMENT;
+    }
+    if (channels < 1 || channels > GSB_MAX_FEATURE_CHANNELS) {
+        set_error("gsb_render_features: channels %d outside 1..%d", channels, GSB_MAX_FEATURE_CHANNELS);
+        return GSB_ERR_ARGUMENT;
+    }
+    if (misaligned(features) || misaligned(out)) {
+        set_error("gsb_render_features: features and out must be 4-byte aligned float pointers");
+        return GSB_ERR_ARGUMENT;
+    }
+    FeatArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = width; a.H = height; a.gx = (width + TILE - 1) / TILE; a.gy = (height + TILE - 1) / TILE; a.V = V; a.C = channels; a.P = P;
+    a.features = features; a.out = out;
+    const size_t npix = (size_t)height * width;
+    for (int v = 0; v < V; ++v) {
+        // the IMAGE buffer holds final_T and n_contrib of npix pixels each (carve_image): a smaller one is another image size
+        if (!feat_view(states[v], P, a.gx * a.gy, a.view[v]) || !states[v].image ||
+            (const char *)states[v].n_contrib + npix * sizeof(uint32_t) > (const char *)states[v].image + states[v].image_bytes) {
+            set_error("gsb_render_features: state %d is not a forward of %d gaussians over %d x %d pixels", v, P, width, height);
+            return GSB_ERR_ARGUMENT;
+        }
+    }
+    return launch_render_features(a, false, static_cast<cudaStream_t>(cuda_stream));
 }
 
 static int check_batch(int32_t V, const GsbSettings *s, const GsbInputs *in, CamArgsBatch &cb) {
@@ -748,13 +845,21 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
                                const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth, const GsbGrads *grads,
                                int32_t accumulate, int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx, gsb_alloc_fn alloc,
                                void *alloc_ctx, cudaStream_t stream, const GsbPeerTable *peers = nullptr,
-                               const GsbCameraGrads *cam_grads = nullptr, const float *dL_dalpha = nullptr) {
+                               const GsbCameraGrads *cam_grads = nullptr, const float *dL_dalpha = nullptr,
+                               const GsbFeatures *feat = nullptr) {
     CamArgsBatch cb;
     int rc = check_batch(V, s, in, cb);
     if (rc) return rc;
     bool want_cam = false;
     rc = check_cam_grads("gsb_backward_batch_camera", cam_grads, want_cam);
     if (rc) return rc;
+    bool want_feat = false;
+    rc = check_features("gsb_backward_batch_features", feat, in->P, want_feat);
+    if (rc) return rc;
+    if (feat && (peers || n_chunks > 1 || on_chunk)) {
+        set_error("gsb_backward_batch_features: features are not available on the chunked or peer backward");
+        return GSB_ERR_ARGUMENT;
+    }
     const bool debug = s[0].debug != 0;
     const CamArgs &c0 = cb.cam[0];
     const int P = in->P;
@@ -776,6 +881,8 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
     float *dacc = static_cast<float *>(do_alloc(alloc, alloc_ctx, GSB_BUF_SCRATCH0, dacc_bytes));
     if (!dacc) return GSB_ERR_ALLOC;
     GSB_CUDA(cudaMemsetAsync(dacc, 0, dacc_bytes, stream));
+    if (feat && feat->dL_dfeatures && !accumulate)
+        GSB_CUDA(cudaMemsetAsync(feat->dL_dfeatures, 0, (size_t)P * feat->channels * sizeof(float), stream));
     const size_t sv_splat = V > 1 ? (size_t)((const float4 *)states[1].splat - (const float4 *)states[0].splat) : 0;
     if (any) {
         RenderBwdArgs ra;
@@ -794,6 +901,21 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
         ra.final_T = states[0].final_T; ra.dL_dalpha = dL_dalpha;     // final_T and n_contrib share the IMAGE stride sv_image
         rc = launch_render_bwd(ra, debug, stream);
         if (rc) return rc;
+        if (want_feat) {     // adds into the same accumulator rows, view v at rows v * P + id
+            FeatArgs fa;
+            memset(&fa, 0, sizeof(fa));
+            fa.W = c0.W; fa.H = c0.H; fa.gx = c0.gx; fa.gy = c0.gy; fa.V = V; fa.C = feat->channels; fa.P = P;
+            for (int v = 0; v < V; ++v) {
+                if (!feat_view(states[v], P, c0.gx * c0.gy, fa.view[v])) {
+                    set_error("gsb_backward_batch_features: state %d has no binning", v);
+                    return GSB_ERR_ARGUMENT;
+                }
+            }
+            fa.features = feat->features; fa.out_features = feat->out_features; fa.dL_dout = feat->dL_dout_features;
+            fa.dacc = dacc; fa.dL_dfeatures = feat->dL_dfeatures;
+            rc = launch_render_features_bwd(fa, debug, stream);
+            if (rc) return rc;
+        }
     }
     PreBwdArgs pa;
     pa.P = P; pa.means = in->means3D; pa.shs = in->shs; pa.opac = in->opacities; pa.scales = in->scales; pa.rots = in->rotations;
@@ -905,6 +1027,27 @@ int32_t gsb_backward_batch_alpha(int32_t V, const GsbSettings *s, const GsbInput
     if (peers) { accumulate = 1; n_chunks = 1; on_chunk = nullptr; }
     return backward_batch_impl(V, s, in, states, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate, n_chunks, on_chunk,
                                chunk_ctx, alloc, alloc_ctx, static_cast<cudaStream_t>(cuda_stream), peers, cam_grads, dL_dalpha);
+}
+
+int32_t gsb_backward_batch_features(int32_t V, const GsbSettings *s, const GsbInputs *in, const GsbState *states, const float *out_color,
+                                    const float *out_invdepth, const float *dL_dcolor, const float *dL_dinvdepth, const float *dL_dalpha,
+                                    const GsbGrads *grads, const GsbCameraGrads *cam_grads, const GsbFeatures *features,
+                                    const GsbPeerTable *peers, int32_t accumulate, int32_t n_chunks, gsb_chunk_fn on_chunk,
+                                    void *chunk_ctx, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {
+    if (!s || !in || !states || !out_color || !out_invdepth || !dL_dcolor || !grads || !alloc || in->P <= 0 || n_chunks < 1 ||
+        n_chunks > 64) {
+        set_error("gsb_backward_batch_features: NULL argument, empty input or n_chunks outside 1..64");
+        return GSB_ERR_ARGUMENT;
+    }
+    if (misaligned(dL_dalpha)) {
+        set_error("gsb_backward_batch_features: dL_dalpha must be a 4-byte aligned float pointer");
+        return GSB_ERR_ARGUMENT;
+    }
+    // gsb_backward_batch_alpha's mode selection (backward_batch_impl refuses features with chunks or peers)
+    if (peers) { accumulate = 1; n_chunks = 1; on_chunk = nullptr; }
+    return backward_batch_impl(V, s, in, states, out_color, out_invdepth, dL_dcolor, dL_dinvdepth, grads, accumulate, n_chunks, on_chunk,
+                               chunk_ctx, alloc, alloc_ctx, static_cast<cudaStream_t>(cuda_stream), peers, cam_grads, dL_dalpha,
+                               features);
 }
 
 // ---- peer memory (one process per GPU of a node): allocation + CUDA IPC, for the fused reduce-scatter ----

@@ -7,6 +7,7 @@ namespace gsb {
 
 // per-gaussian gradient accumulator written by the backward blend kernel (float, 48 B stride):
 //   0..4 raw moments of t = dL/d(power): sum t dx, t dy, t dx^2, t dx dy, t dy^2   5 opacity  6,7,8 rgb  9 inverse depth  10,11 pad
+// (the feature pass, features.cu, adds its terms of a feature loss into 0..5 of the same rows)
 constexpr int DACC_STRIDE = 12;
 
 // ---- view-batch variants: per-view arrays are laid out [V][...] with uniform strides (in elements) ----
@@ -130,6 +131,27 @@ struct AlphaArgs {
     float *out;           // [V][npix]
 };
 
+// Rendered feature maps (features.cu, DESIGN.md section 7.7): F[v][c][p] = sum_k w_k(p) features[id_k][c] with the forward's blend
+// weights, channels in groups of 4 or 8 (blockIdx.z) and views in blockIdx.y.  Every view is one forward state of its own
+// (any forward entry point); the backward adds its moment and opacity terms into rows view * P + id of `dacc` (the same rows
+// render_bwd_kernel fills) and dL/dfeatures, summed over the views, into dL_dfeatures.
+constexpr int FEAT_MAX_CHANNELS = 128;
+struct FeatView {
+    const uint2 *ranges;
+    const uint32_t *point_list, *tile_order;
+    const float4 *splat;
+    const uint32_t *n_contrib;
+};
+struct FeatArgs {
+    int W, H, gx, gy, V, C, P;
+    FeatView view[GSB_MAX_VIEWS];
+    const float *features;                  // [P, C]
+    float *out;                             // forward: [V, C, H*W]
+    const float *out_features, *dL_dout;    // backward: the forward's output and its gradient, [V, C, H*W]
+    float *dacc;                            // backward: [V * P, DACC_STRIDE], zeroed by the caller
+    float *dL_dfeatures;                    // backward: [P, C], added into; NULL = not requested
+};
+
 // split: a.shs / a.rest are the split SH input (see PreFwdArgs)
 int launch_preprocess_fwd(const CamArgs &ca, const PreFwdArgs &a, bool split, bool debug, cudaStream_t stream);
 int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool split, bool accumulate, bool debug, cudaStream_t stream);
@@ -151,6 +173,8 @@ int launch_tile_ranges(const uint32_t *sorted_tiles, int64_t D, const unsigned l
 int launch_render_fwd(const RenderFwdArgs &a, bool debug, cudaStream_t stream);
 int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream);
 int launch_alpha(const AlphaArgs &a, bool debug, cudaStream_t stream);
+int launch_render_features(const FeatArgs &a, bool debug, cudaStream_t stream);
+int launch_render_features_bwd(const FeatArgs &a, bool debug, cudaStream_t stream);
 int launch_tile_order(const uint2 *ranges, int V, int num_tiles, uint32_t *order, bool debug, cudaStream_t stream);
 int launch_l1_loss_grad(const float *img, const float *gt, int64_t n, float scale, float *grad, float *loss_accum,
                         cudaStream_t stream);

@@ -91,6 +91,14 @@ class _CameraGrads(Structure):       # GsbCameraGrads
     _fields_ = [("dL_dviewmatrix", c_void_p), ("dL_dprojmatrix", c_void_p), ("dL_dcampos", c_void_p), ("dL_dbg", c_void_p)]
 
 
+class _Features(Structure):          # GsbFeatures
+    _fields_ = [("channels", c_int32), ("features", c_void_p), ("out_features", c_void_p), ("dL_dout_features", c_void_p),
+                ("dL_dfeatures", c_void_p)]
+
+
+MAX_FEATURE_CHANNELS = 128          # GSB_MAX_FEATURE_CHANNELS
+
+
 class _SparseAdamGroup(Structure):   # GsbSparseAdamGroup
     _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p), ("width", c_int32),
                 ("lr", c_float), ("eps", c_float)]
@@ -138,6 +146,17 @@ def _load(path: Optional[str] = None):
                                              c_void_p, c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads),
                                              POINTER(_PeerTable), c_int32, c_int32, _CHUNK_FN, c_void_p, _ALLOC_FN, c_void_p,
                                              c_void_p]
+    lib.gsb_render_features.restype = c_int32
+    lib.gsb_render_features.argtypes = [c_int32, POINTER(_State), c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.gsb_backward_features.restype = c_int32
+    lib.gsb_backward_features.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), POINTER(_State), c_void_p,
+                                          c_void_p, c_void_p, c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads),
+                                          POINTER(_Features), c_int32, _ALLOC_FN, c_void_p, c_void_p]
+    lib.gsb_backward_batch_features.restype = c_int32
+    lib.gsb_backward_batch_features.argtypes = [c_int32, POINTER(_Settings), POINTER(_Inputs), POINTER(_State), c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads),
+                                                POINTER(_Features), POINTER(_PeerTable), c_int32, c_int32, _CHUNK_FN, c_void_p,
+                                                _ALLOC_FN, c_void_p, c_void_p]
     lib.gsb_sparse_adam_step.restype = c_int32
     lib.gsb_sparse_adam_step.argtypes = [POINTER(_SparseAdamGroup), c_int32, c_void_p, c_int64, c_float, c_float, c_void_p]
     lib.gsb_forward_batch.restype = c_int32
@@ -602,6 +621,49 @@ def _alpha_impl(states, height: int, width: int, device) -> torch.Tensor:
     return out[0] if one else out
 
 
+def check_features(features, P: int, device) -> None:
+    """Raises ValueError unless ``features`` is a [P, C] tensor with 1 <= C <= MAX_FEATURE_CHANNELS on ``device``."""
+    if not isinstance(features, torch.Tensor) or features.dim() != 2:
+        raise ValueError(f"features must be a 2-D tensor [P, C]; got {type(features).__name__} "
+                         f"{tuple(features.shape) if isinstance(features, torch.Tensor) else ''}")
+    if int(features.shape[0]) != int(P):
+        raise ValueError(f"features has {int(features.shape[0])} rows, the gaussians number {int(P)}")
+    if not 1 <= int(features.shape[1]) <= MAX_FEATURE_CHANNELS:
+        raise ValueError(f"features has {int(features.shape[1])} channels, 1..{MAX_FEATURE_CHANNELS} are supported")
+    if features.device != torch.device(device):
+        raise ValueError(f"features live on {features.device}, the gaussians on {device}")
+
+
+def _features_impl(states, height: int, width: int, features: torch.Tensor, device) -> torch.Tensor:
+    """Rendered feature maps (gsb_render_features) of the forward states ``states`` (a ``_State`` or a ctypes array of them) for
+    ``features`` [P, C] float32 contiguous: [V,C,H,W] for an array, [C,H,W] for one state.  One launch, no synchronisation."""
+    one = isinstance(states, _State)
+    V = 1 if one else len(states)
+    P, C = int(features.shape[0]), int(features.shape[1])
+    out = torch.empty((V, C, int(height), int(width)), dtype=torch.float32, device=device)
+    with _device_ctx(device):
+        rc = _C.gsb_render_features(V, byref(states) if one else states, int(height), int(width), P, C,
+                                    features.data_ptr() if P > 0 else None, out.data_ptr(), _current_stream(device))
+    _check(rc)
+    return out[0] if one else out
+
+
+def _feature_term(feats: Optional[dict]):
+    """GsbFeatures over ``feats`` = {"features": [P,C], "out": forward output, "grad": dL/d output or None, "dL_dfeatures":
+    [P,C] or None}, all float32 contiguous; None for no feature term."""
+    if feats is None:
+        return None
+    f = feats["features"]
+    ft = _Features()
+    ft.channels = int(f.shape[1])
+    ft.features = f.data_ptr() if f.numel() > 0 else None
+    ft.out_features = feats["out"].data_ptr()
+    ft.dL_dout_features = _ptr(feats.get("grad"))
+    d = feats.get("dL_dfeatures")
+    ft.dL_dfeatures = d.data_ptr() if d is not None and d.numel() > 0 else None
+    return ft
+
+
 CAMERA_KEYS = ("viewmatrix", "projmatrix", "campos", "bg")     # GsbCameraGrads, in field order
 _CAMERA_NUMEL = dict(viewmatrix=16, projmatrix=16, campos=3, bg=3)
 
@@ -627,13 +689,14 @@ def _camera_grads(cam_grads: Optional[dict], V: Optional[int] = None):
 def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                    out_color, out_invdepth, grad_color, grad_invdepth, grads: dict, accumulate: bool,
                    accumulate_means2D: Optional[bool] = None, dc=None, cam_grads: Optional[dict] = None,
-                   grad_alpha: Optional[torch.Tensor] = None):
+                   grad_alpha: Optional[torch.Tensor] = None, feats: Optional[dict] = None):
     """grads: tensors to fill (accumulate=False) or add into (accumulate=True).  The C ABI has one accumulate
     switch; a per-view means2D buffer (accumulate_means2D=False while the rest accumulates) is zeroed here.
     ``dc``: split SH input (gsb_backward_split_sh); ``sh`` is the rest, grads["dc"] / grads["shs"] receive their gradients.
     ``cam_grads``: {"viewmatrix": [16], "projmatrix": [16], "campos": [3], "bg": [3]} float32 tensors (any subset) that receive
     the camera gradient under the same accumulate switch (gsb_backward_camera).  ``grad_alpha``: dL/d rendered alpha [1,H,W]
-    float32 contiguous, or None (gsb_backward_alpha; None takes the calls above)."""
+    float32 contiguous, or None (gsb_backward_alpha; None takes the calls above).  ``feats``: the feature term (_feature_term;
+    gsb_backward_features), or None."""
     if accumulate and accumulate_means2D is False and grads.get("means2D") is not None:
         grads["means2D"].zero_()
     dev = means3D.device
@@ -651,7 +714,14 @@ def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rot
         stream = _current_stream(dev)
         arena = _Arena(dev, stream)
         cg = _camera_grads(cam_grads)
-        if grad_alpha is not None:
+        ft = _feature_term(feats)
+        if ft is not None:
+            sp = _split_sh(dc, sh, grads) if dc is not None else None
+            rc = _C.gsb_backward_features(byref(cs), byref(ci), byref(sp) if sp is not None else None, byref(pack["state"]),
+                                          out_color.data_ptr(), out_invdepth.data_ptr(), grad_color.data_ptr(), _ptr(grad_invdepth),
+                                          _ptr(grad_alpha), byref(g), byref(cg) if cg is not None else None, byref(ft),
+                                          int(bool(accumulate)), arena.cb, None, stream)
+        elif grad_alpha is not None:
             sp = _split_sh(dc, sh, grads) if dc is not None else None
             rc = _C.gsb_backward_alpha(byref(cs), byref(ci), byref(sp) if sp is not None else None, byref(pack["state"]),
                                        out_color.data_ptr(), out_invdepth.data_ptr(), grad_color.data_ptr(), _ptr(grad_invdepth),
@@ -726,7 +796,8 @@ def capacity_for(count: int) -> int:
 
 def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, rotations, out_color, out_invdepth,
                          grad_color, grad_invdepth, grads: dict, accumulate: bool, n_chunks: int = 1, on_chunk=None, peers=None,
-                         cam_grads: Optional[dict] = None, grad_alpha: Optional[torch.Tensor] = None):
+                         cam_grads: Optional[dict] = None, grad_alpha: Optional[torch.Tensor] = None,
+                         feats: Optional[dict] = None):
     """View-batch backward (gsb_backward_batch).  grads: tensors holding / receiving the gradient SUMMED over the views
     (means2D, if present, is [V,P,3] and per view).  ``n_chunks`` > 1: gsb_backward_batch_chunked -- the last kernel runs in
     gaussian-range chunks and ``on_chunk(chunk, p_begin, p_end)`` is called after each chunk has been enqueued (rows
@@ -735,13 +806,17 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
     gaussian_renderer.peer.PeerGradientBucket drives the protocol around it).  ``cam_grads``: {"viewmatrix": [V,16],
     "projmatrix": [V,16], "campos": [V,3], "bg": [V,3]} float32 tensors (any subset) receiving each view's camera gradient
     (gsb_backward_batch_camera); not with ``n_chunks`` > 1, ``on_chunk`` or ``peers``.  ``grad_alpha``: dL/d rendered alpha
-    [V,1,H,W] float32 contiguous, or None; with it every mode goes through gsb_backward_batch_alpha."""
+    [V,1,H,W] float32 contiguous, or None; with it every mode goes through gsb_backward_batch_alpha.  ``feats``: the feature
+    term (_feature_term over [V,C,H,W] maps; gsb_backward_batch_features), plain and camera modes only."""
     dev = means3D.device
     V, P = pack["V"], int(means3D.shape[0])
     cg = _camera_grads(cam_grads, V)
     if cg is not None and (peers is not None or n_chunks > 1 or on_chunk is not None):
         raise ValueError("camera gradients are not available on the chunked or peer view-batch backward: the per-view sum "
                          "would have to span gaussian chunks or ranks")
+    ft = _feature_term(feats)
+    if ft is not None and (peers is not None or n_chunks > 1 or on_chunk is not None):
+        raise ValueError("features are not available on the chunked or peer view-batch backward")
     with _device_ctx(dev):
         keep = []
         cs = (_Settings * V)(*[_c_settings(rs, pack["sh_coeffs"], keep) for rs in settings_list])
@@ -766,7 +841,13 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
                     on_chunk(int(chunk), int(p0), int(p1))
             except Exception as e:  # never let an exception cross the C ABI
                 err.append(e)
-        if grad_alpha is not None:
+        if ft is not None:
+            rc = _C.gsb_backward_batch_features(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
+                                                grad_color.data_ptr(), _ptr(grad_invdepth), _ptr(grad_alpha), byref(g),
+                                                byref(cg) if cg is not None else None, byref(ft), None, int(bool(accumulate)), 1,
+                                                _CHUNK_FN(), None, arena.cb, None, stream)
+            _check(rc, arena)
+        elif grad_alpha is not None:
             chunked = pt is None and (n_chunks > 1 or on_chunk is not None)
             cb = _CHUNK_FN(_cb) if chunked else _CHUNK_FN()     # NULL callback
             rc = _C.gsb_backward_batch_alpha(V, cs, byref(ci), pack["states"], out_color.data_ptr(), out_invdepth.data_ptr(),
@@ -801,7 +882,7 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, dc=None, return_alpha=False):
+                        raster_settings, dc=None, return_alpha=False, features=None):
     """``dc`` (optional): split SH input -- ``dc`` [P,1,3] holds the DC coefficient and ``sh`` [P,M-1,3] the others (M-1 may
     be 0); the result equals that of ``sh = cat((dc, sh), 1)`` without the concatenation.
 
@@ -811,9 +892,17 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
     ``return_alpha=True``: the result is (color, radii, invdepth, alpha[1,H,W]) with alpha = 1 - final transmittance (gsb_alpha;
     definition in include/gs_b200.h), differentiable w.r.t. every gaussian input and the camera tensors.  One extra launch in the
-    forward; a backward in which alpha's gradient is unused (None) is the plain one."""
+    forward; a backward in which alpha's gradient is unused (None) is the plain one.
+
+    ``features`` [P, C] (1 <= C <= MAX_FEATURE_CHANNELS, view-independent): one more trailing output, the feature map [C,H,W]
+    = sum_k alpha_k T_k features[k] with the forward's blend weights and background 0 (gsb_render_features; definition in
+    include/gs_b200.h).  Its gradient reaches ``features`` and every gaussian and camera input.  One extra launch in the forward,
+    one in a backward that uses the map's gradient; without ``features`` the call is unchanged.  Bad shapes raise ValueError."""
+    if features is not None:
+        check_features(features, int(means3D.shape[0]), means3D.device)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings, dc, bool(return_alpha), *_camera_inputs(raster_settings))
+                                     cov3Ds_precomp, raster_settings, dc, bool(return_alpha), features,
+                                     *_camera_inputs(raster_settings))
 
 
 def _camera_inputs(rs) -> tuple:
@@ -827,7 +916,7 @@ def _camera_inputs(rs) -> tuple:
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, dc=None, return_alpha=False, *camera):
+                raster_settings, dc=None, return_alpha=False, features=None, *camera):
         # camera: the settings' (viewmatrix, projmatrix, campos, bg) as inputs of their own (rasterize_gaussians), or ()
         args = [_f32c(means3D), _f32c(sh), _f32c(colors_precomp), _f32c(opacities), _f32c(scales), _f32c(rotations),
                 _f32c(cov3Ds_precomp)]
@@ -840,7 +929,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             color, radii, invdepth, pack = _forward_impl(*args, raster_settings, dc=dcc)
         except Exception:
             if raster_settings.debug:
-                dump = args + ([dcc] if dc is not None else [])
+                dump = args + ([dcc] if dc is not None else []) + ([features] if features is not None else [])
                 torch.save([a.detach().cpu() if a is not None else None for a in dump], "snapshot_fw.dump")
                 print("\nAn error occured in forward. Writing snapshot_fw.dump for debugging.")
             raise
@@ -849,17 +938,29 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.pack = pack
         ctx.shapes = dict(means2D=None if means2D is None else tuple(means2D.shape), opacities=tuple(opacities.shape),
                           sh=None if sh is None else tuple(sh.shape), dc=None if dc is None else tuple(dc.shape))
+        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
+        fc = fmap = None
+        if features is not None:
+            fc = features.detach().float().contiguous()
+            fmap = _features_impl(pack["state"], H, W, fc, color.device)
         ctx.save_for_backward(*[a if a is not None else torch.empty(0) for a in args], color, invdepth,
-                              dcc if dcc is not None else torch.empty(0))
+                              dcc if dcc is not None else torch.empty(0), *((fc, fmap) if fc is not None else ()))
         ctx.mark_non_differentiable(radii)
         ctx.camera = [(tuple(t.shape), t.dtype) for t in camera]
+        ctx.return_alpha = bool(return_alpha)
+        ctx.has_features = features is not None
+        out = (color, radii, invdepth)
         if return_alpha:
-            alpha = _alpha_impl(pack["state"], int(raster_settings.image_height), int(raster_settings.image_width), color.device)
-            return color, radii, invdepth, alpha
-        return color, radii, invdepth
+            out += (_alpha_impl(pack["state"], H, W, color.device),)
+        if features is not None:
+            out += (fmap,)
+        return out
 
     @staticmethod
-    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth, grad_out_alpha=None):
+    def backward(ctx, grad_out_color, _grad_radii, grad_out_depth, *grad_extra):
+        # grad_extra: the gradients of the optional outputs, (alpha)? (features)?
+        grad_out_alpha = grad_extra[0] if ctx.return_alpha else None
+        grad_out_feat = grad_extra[-1] if ctx.has_features else None
         rs = ctx.raster_settings
         saved = [t if t.numel() > 0 else None for t in ctx.saved_tensors[:7]]
         means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp = saved
@@ -885,9 +986,9 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads["scales"] = new(P, 3)
             grads["rotations"] = new(P, 4)
         cam_grads = {k: torch.empty(_CAMERA_NUMEL[k], dtype=torch.float32, device=dev)
-                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[11 + j]}
-        if grad_out_color is None and grad_out_depth is None and grad_out_alpha is None:
-            return (None,) * (11 + len(ctx.camera))
+                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[12 + j]}
+        if grad_out_color is None and grad_out_depth is None and grad_out_alpha is None and grad_out_feat is None:
+            return (None,) * (12 + len(ctx.camera))
         gc = _f32c(grad_out_color)
         if gc is None:
             gc = torch.zeros((3, int(rs.image_height), int(rs.image_width)), dtype=torch.float32, device=dev)
@@ -895,15 +996,22 @@ class _RasterizeGaussians(torch.autograd.Function):
         ga = _f32c(grad_out_alpha)
         if dc is None and "dc" in grads:                         # P == 0
             grads["dc"].zero_()
+        feats = None
+        if grad_out_feat is not None:
+            fc, fmap = ctx.saved_tensors[10], ctx.saved_tensors[11]
+            feats = dict(features=fc, out=fmap, grad=_f32c(grad_out_feat),
+                         dL_dfeatures=torch.empty(fc.shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[11] else None)
         try:
             _backward_impl(ctx.pack, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc, cam_grads=cam_grads, grad_alpha=ga)
+                           out_color, out_invdepth, gc, gd, grads, accumulate=False, dc=dc, cam_grads=cam_grads, grad_alpha=ga,
+                           feats=feats)
         except Exception:
             if rs.debug:
                 split = [ctx.saved_tensors[9].cpu()] if ctx.shapes["dc"] is not None else []
                 camera = [getattr(rs, k).detach().cpu() for k in CAMERA_KEYS] if ctx.camera else []
                 alpha = [ga.cpu()] if ga is not None else []
-                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()] + camera + alpha,
+                feat = [feats["features"].cpu(), feats["grad"].cpu()] if feats is not None else []
+                torch.save([t.detach().cpu() for t in ctx.saved_tensors[:9]] + split + [gc.cpu()] + camera + alpha + feat,
                            "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
             raise
@@ -912,7 +1020,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                       for k, (shape, dtype) in zip(CAMERA_KEYS, ctx.camera))
         return (grads["means3D"], grads["means2D"] if ctx.shapes["means2D"] is not None else None, grads.get("shs"),
                 grads.get("colors_precomp"), g_op, grads.get("scales"), grads.get("rotations"),
-                grads.get("cov3D_precomp"), None, grads.get("dc"), None) + g_cam
+                grads.get("cov3D_precomp"), None, grads.get("dc"), None,
+                feats["dL_dfeatures"] if feats is not None else None) + g_cam
 
 
 class GaussianRasterizer(nn.Module):
@@ -936,10 +1045,11 @@ class GaussianRasterizer(nn.Module):
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, dc=None, return_alpha=False):
+                cov3D_precomp=None, dc=None, return_alpha=False, features=None):
         """``dc``: the split SH input of the accel branch (gaussian_renderer/__init__.py:90-100) -- ``dc`` [P,1,3] is the DC
         coefficient and ``shs`` [P,M-1,3] the others (may have zero coefficients); gradients come back in the same split.
-        ``return_alpha=True``: also returns the rendered alpha [1,H,W] (rasterize_gaussians)."""
+        ``return_alpha=True``: also returns the rendered alpha [1,H,W] (rasterize_gaussians).  ``features`` [P,C]: also returns
+        the feature map [C,H,W], last (rasterize_gaussians)."""
         rs = self.raster_settings
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
@@ -949,7 +1059,7 @@ class GaussianRasterizer(nn.Module):
         if dc is not None and colors_precomp is not None:
             raise Exception("dc is the SH DC coefficient: it goes with shs, not with precomputed colors!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   rs, dc, return_alpha)
+                                   rs, dc, return_alpha, features)
 
 
 # SparseGaussianAdam: bound here only on request (module docstring); sparse_adam.py is importable either way

@@ -48,10 +48,13 @@ def _eval_sh(deg, sh, dirs):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, separate_sh=False,
-           override_color=None, use_trained_exp=False, return_alpha=False):
+           override_color=None, use_trained_exp=False, return_alpha=False, features=None):
     """Same contract as the reference's render(): returns
     {"render", "viewspace_points", "visibility_filter", "radii", "depth"}.  ``return_alpha=True`` adds "alpha": the rendered
-    accumulated opacity [1,H,W] (1 - final transmittance, differentiable; the exposure of ``use_trained_exp`` does not apply)."""
+    accumulated opacity [1,H,W] (1 - final transmittance, differentiable; the exposure of ``use_trained_exp`` does not apply).
+    ``features`` [P,C] (per-gaussian, view-independent, 1 <= C <= 128) adds "features": the feature map [C,H,W] composited
+    with the same blend weights over a zero background, differentiable w.r.t. ``features`` and the gaussians (no exposure,
+    no clamp)."""
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -90,7 +93,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         colors_precomp = override_color
 
     out = rasterizer(means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors_precomp, opacities=pc.get_opacity,
-                     scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, dc=dc, return_alpha=return_alpha)
+                     scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, dc=dc, return_alpha=return_alpha,
+                     features=features)
     rendered_image, radii, depth_image = out[:3]
 
     if use_trained_exp:
@@ -102,6 +106,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
               "visibility_filter": (radii > 0).nonzero(), "radii": radii, "depth": depth_image}
     if return_alpha:
         result["alpha"] = out[3]
+    if features is not None:
+        result["features"] = out[-1]
     return result
 
 
@@ -188,7 +194,7 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                           scaling_modifier: float = 1.0, densify_stats: Optional[dict] = None,
                           keep_images: bool = False, loss_returns_grad: bool = False, batched: bool = True,
                           overwrite: bool = False, capacity: Optional[AsyncCapacity] = None, grad_chunks: int = 1,
-                          on_grad_chunk=None, peers=None, with_alpha: bool = False) -> dict:
+                          on_grad_chunk=None, peers=None, with_alpha: bool = False, features=None) -> dict:
     """Fused view-batch training step: forward + loss + backward for every camera, with the per-gaussian
     gradients of ALL views summed in place.
 
@@ -223,6 +229,12 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     ``(loss, dL/d image, dL/d invdepth | None, dL/d alpha | None)``.  The alpha gradient goes into the same backward call in every
     mode (batched or not, sync or async, chunked, peers); a view batch in which no view returns one takes the plain backward.
     ``keep_images=True`` also returns "alphas".
+
+    ``features`` [P,C] (per-gaussian, view-independent; a leaf or not): ``loss_fn`` also receives the view's feature map [C,H,W]
+    (render(features=...)) as the keyword ``features``; with ``loss_returns_grad=True`` it may return a fifth element,
+    ``dL/d feature map | None`` (the fourth, alpha's, may be None).  dL/dfeatures, summed over the views, goes into ``features``
+    like a gaussian input's gradient, and the map's gradient into the same backward call.  Not with ``grad_chunks`` > 1,
+    ``on_grad_chunk`` or ``peers`` (ValueError).  ``keep_images=True`` also returns "features" (the maps).
     """
     takes_grad_out = False
     if loss_returns_grad:
@@ -244,6 +256,39 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
 
     targets = {k: grad_target(v) for k, v in inputs.items()}
     grads = {k: tv[0] for k, tv in targets.items()}
+    fc = f_target = None
+    if features is not None:
+        _dgr.check_features(features, P, dev)
+        if grad_chunks > 1 or on_grad_chunk is not None or peers is not None:
+            raise ValueError("render_views_backward: features cannot be combined with grad_chunks > 1, on_grad_chunk or peers")
+        fc = features.detach().float().contiguous()
+        if features.requires_grad:
+            f_target = grad_target(features)
+            if f_target[1] and f_target[0].dtype != torch.float32:     # the kernels add float32 only
+                f_target = (torch.zeros(features.shape, dtype=torch.float32, device=dev), False)
+    fmaps = []
+
+    def feature_term(fmap, g_feat):
+        """the backward's feature term (None: no view of the call returned a feature-map gradient)"""
+        if g_feat is None:
+            return None
+        return dict(features=fc, out=fmap, grad=g_feat, dL_dfeatures=f_target[0] if f_target is not None else None)
+
+    def view_loss(img_in, dep_in, vi, extra, grad_out=None):
+        """(loss, dL/d image, dL/d invdepth, dL/d alpha, dL/d feature map) of one view; extra: loss_fn's keyword inputs"""
+        if loss_returns_grad:
+            res = loss_fn(img_in, dep_in, vi, grad_out=grad_out, **extra) if grad_out is not None else \
+                loss_fn(img_in, dep_in, vi, **extra)
+            res = tuple(res) + (None,) * (5 - len(res))
+            return res[0], res[1], res[2], res[3] if with_alpha else None, res[4] if fc is not None else None
+        img = img_in.detach().requires_grad_(True)
+        dep = dep_in.detach().requires_grad_(True)
+        extra = {a: t.detach().requires_grad_(True) for a, t in extra.items()}
+        with torch.enable_grad():
+            loss = loss_fn(img.clamp(0, 1), dep, vi, **extra)
+        g = torch.autograd.grad(loss, (img, dep, *extra.values()), allow_unused=True)
+        ge = dict(zip(extra.keys(), g[2:]))
+        return loss, g[0], g[1], ge.get("alpha"), ge.get("features")
     if densify_stats is not None:
         m2d = torch.empty((P, 3), dtype=torch.float32, device=dev)
     c = {k: _dgr._f32c(v.detach()) for k, v in inputs.items()}
@@ -285,26 +330,16 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                 capacity.learn(pack["num_rendered"])
             num_rendered.extend(pack["num_rendered"])
             alpha = _dgr._alpha_impl(pack["states"], int(color.shape[-2]), int(color.shape[-1]), dev) if with_alpha else None
+            fmap = _dgr._features_impl(pack["states"], int(color.shape[-2]), int(color.shape[-1]), fc, dev) if fc is not None else None
             g_color = torch.empty_like(color)
-            g_depth = g_alpha = None
+            g_depth = g_alpha = g_feat = None
             for k in range(len(chunk)):
                 vi = c0 + k
                 akw = dict(alpha=alpha[k]) if with_alpha else {}
-                g_al = None
-                if loss_returns_grad:
-                    res = loss_fn(color[k], invdepth[k], vi, grad_out=g_color[k], **akw) if takes_grad_out else \
-                        loss_fn(color[k], invdepth[k], vi, **akw)
-                    loss, g_img = res[0], res[1]
-                    g_dep = res[2] if len(res) > 2 else None
-                    g_al = res[3] if with_alpha and len(res) > 3 else None
-                else:
-                    img = color[k].detach().requires_grad_(True)
-                    dep = invdepth[k].detach().requires_grad_(True)
-                    akw = {a: t.detach().requires_grad_(True) for a, t in akw.items()}
-                    with torch.enable_grad():
-                        loss = loss_fn(img.clamp(0, 1), dep, vi, **akw)
-                    g_img, g_dep, *g_al = torch.autograd.grad(loss, (img, dep, *akw.values()), allow_unused=True)
-                    g_al = g_al[0] if g_al else None
+                if fc is not None:
+                    akw["features"] = fmap[k]
+                loss, g_img, g_dep, g_al, g_fe = view_loss(color[k], invdepth[k], vi, akw,
+                                                           grad_out=g_color[k] if takes_grad_out else None)
                 if g_img is None:
                     g_color[k].zero_()
                 elif g_img.data_ptr() != g_color[k].data_ptr():
@@ -317,11 +352,17 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                     if g_alpha is None:
                         g_alpha = torch.zeros_like(alpha)
                     g_alpha[k].copy_(g_al.reshape(alpha[k].shape))
+                if g_fe is not None:
+                    if g_feat is None:
+                        g_feat = torch.zeros_like(fmap)
+                    g_feat[k].copy_(g_fe.reshape(fmap[k].shape))
                 losses.append(loss.detach().reshape(()))
                 if keep_images:
                     images.append(color[k].detach())
                     if with_alpha:
                         alphas.append(alpha[k])
+                    if fc is not None:
+                        fmaps.append(fmap[k])
             vg = dict(grads)
             if densify_stats is not None:
                 vg["means2D"] = torch.empty((len(chunk), P, 3), dtype=torch.float32, device=dev)
@@ -330,7 +371,7 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
             _dgr._backward_batch_impl(pack, rss, c["means3D"], c["shs"], c["opacities"], c["scales"], c["rotations"], color,
                                       invdepth, g_color, g_depth, vg, accumulate=not (overwrite and c0 == 0),
                                       n_chunks=grad_chunks if last_chunk else 1, on_chunk=on_grad_chunk if last_chunk else None,
-                                      peers=peers, cam_grads=cam_grads, grad_alpha=g_alpha)
+                                      peers=peers, cam_grads=cam_grads, grad_alpha=g_alpha, feats=feature_term(fmap, g_feat))
             chain_camera(rss, cam_grads)
             torch.maximum(radii_max, radii.max(dim=0).values, out=radii_max)
             if densify_stats is not None:
@@ -344,23 +385,13 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                                                           c["rotations"], None, rs)
         num_rendered.append(pack["num_rendered"])
         alpha = _dgr._alpha_impl(pack["state"], int(color.shape[-2]), int(color.shape[-1]), dev) if with_alpha else None
+        fmap = _dgr._features_impl(pack["state"], int(color.shape[-2]), int(color.shape[-1]), fc, dev) if fc is not None else None
         akw = dict(alpha=alpha) if with_alpha else {}
-        g_al = None
-        if loss_returns_grad:
-            res = loss_fn(color, invdepth, vi, **akw)
-            loss, g_img = res[0], res[1]
-            g_dep = res[2] if len(res) > 2 else None
-            g_al = res[3] if with_alpha and len(res) > 3 else None
-        else:
-            img = color.requires_grad_(True)
-            dep = invdepth.requires_grad_(True)
-            akw = {a: t.requires_grad_(True) for a, t in akw.items()}
-            with torch.enable_grad():
-                loss = loss_fn(img.clamp(0, 1), dep, vi, **akw)
-            g_img, g_dep, *g_al = torch.autograd.grad(loss, (img, dep, *akw.values()), allow_unused=True)
-            g_al = g_al[0] if g_al else None
-            if g_img is None:
-                g_img = torch.zeros_like(color)
+        if fc is not None:
+            akw["features"] = fmap
+        loss, g_img, g_dep, g_al, g_fe = view_loss(color, invdepth, vi, akw)
+        if g_img is None and not loss_returns_grad:
+            g_img = torch.zeros_like(color)
         vg = dict(grads)
         if densify_stats is not None:
             vg["means2D"] = m2d
@@ -369,7 +400,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                             color.detach(), invdepth.detach(), _dgr._f32c(g_img), _dgr._f32c(g_dep), vg,
                             accumulate=not (overwrite and vi == 0), accumulate_means2D=False,
                             cam_grads={k: g[0] for k, g in cam_grads.items()} if cam_grads else None,
-                            grad_alpha=_dgr._f32c(g_al.reshape(alpha.shape)) if g_al is not None else None)
+                            grad_alpha=_dgr._f32c(g_al.reshape(alpha.shape)) if g_al is not None else None,
+                            feats=feature_term(fmap, _dgr._f32c(g_fe.reshape(fmap.shape)) if g_fe is not None else None))
         chain_camera([rs], cam_grads)
         torch.maximum(radii_max, radii, out=radii_max)
         if densify_stats is not None:
@@ -382,6 +414,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
             images.append(color.detach())
             if with_alpha:
                 alphas.append(alpha.detach())
+            if fc is not None:
+                fmaps.append(fmap)
     # chain the summed gradient into non-leaf inputs' graphs (one pass, view independent)
     chain_t, chain_g = [], []
     for k, v in inputs.items():
@@ -392,6 +426,9 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     for t, g in cam_chain.values():
         chain_t.append(t)
         chain_g.append(g)
+    if f_target is not None and not f_target[1]:
+        chain_t.append(features)
+        chain_g.append(f_target[0].view_as(features).to(features.dtype))
     if chain_t:
         torch.autograd.backward(chain_t, chain_g)
     if hasattr(pc, "gradients_ready"):      # gaussian_store.GaussianModel: its gradient buffer now belongs to the current parameters
@@ -402,6 +439,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         out["images"] = images
         if with_alpha:
             out["alphas"] = alphas
+        if fc is not None:
+            out["features"] = fmaps
     return out
 
 

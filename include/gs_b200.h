@@ -289,6 +289,54 @@ int32_t gsb_backward_batch_alpha(int32_t V, const GsbSettings *settings, const G
                                  int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx, gsb_alloc_fn alloc,
                                  void *alloc_ctx, void *cuda_stream);
 
+/* Rendered feature maps, DESIGN.md section 7.7: C view-independent per-gaussian channels composited with the forward's own
+ * blend weights,
+ *     F[c][p] = sum_k alpha_k T_k features[id_k][c]
+ * under the forward's rules (the 1/255 cut-off, the 0.99 cap, the T < 1e-4 stop), with background 0 (composite with gsb_alpha
+ * if needed).  Channels 3j..3j+2 equal, bit for bit, the colour output of the same gaussians rendered with colors_precomp =
+ * features[:, 3j:3j+3] and bg = 0.  Channel counts 1..GSB_MAX_FEATURE_CHANNELS.
+ *
+ * gsb_render_features: out [V, channels, height*width] from V forward states (states[v] of any forward call: single view, split
+ * SH, view batch, async view batch; P and height x width must be theirs) and features [P, channels].  One launch, no host
+ * synchronisation; it reads the states' BINNING, GEOM and IMAGE buffers, which must still be alive.  features may be NULL
+ * only when P == 0. */
+#define GSB_MAX_FEATURE_CHANNELS 128
+int32_t gsb_render_features(int32_t V, const GsbState *states, int32_t height, int32_t width, int32_t P, int32_t channels,
+                            const float *features, float *out, void *cuda_stream);
+
+/* The feature term of a backward call.  NULL pointers: no feature loss (dL_dout_features) or no feature gradient
+ * (dL_dfeatures).  A NULL features pointer together with a non-NULL output is an error (unless P == 0). */
+typedef struct GsbFeatures {
+    int32_t channels;                /* C, 1..GSB_MAX_FEATURE_CHANNELS */
+    const float *features;           /* [P, C], as given to gsb_render_features */
+    const float *out_features;       /* [V, C, H*W]: gsb_render_features' output for these states */
+    const float *dL_dout_features;   /* [V, C, H*W] or NULL */
+    float *dL_dfeatures;             /* [P, C] or NULL: written (added with accumulate), summed over the views */
+} GsbFeatures;
+
+/* Backward with a feature term: gsb_backward_alpha (split NULL = joint shs, cam_grads NULL = no camera gradient, dL_dalpha
+ * NULL = no alpha term) plus `features`.  The feature loss enters the per-gaussian gradients (means, opacity, scales /
+ * rotations or cov3D, means2D), the camera gradient and dL_dfeatures; it adds nothing to the colour / SH gradients or dL/dbg.
+ * With features NULL the call is gsb_backward_alpha: the same kernels are launched.  Otherwise one more launch, after the
+ * colour pass, when dL_dout_features is given and the state holds instances. */
+int32_t gsb_backward_features(const GsbSettings *settings, const GsbInputs *in, const GsbSplitSH *split /* NULL = joint shs */,
+                              const GsbState *state, const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                              const float *dL_dinvdepth, const float *dL_dalpha, const GsbGrads *grads,
+                              const GsbCameraGrads *cam_grads, const GsbFeatures *features, int32_t accumulate,
+                              gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
+
+/* View-batch backward with a feature term: gsb_backward_batch_alpha plus `features` (out_features / dL_dout_features
+ * [V, C, H*W]; dL_dfeatures [P, C] is the sum over the views).  With features NULL the call is gsb_backward_batch_alpha in
+ * every mode.  With features, only the plain and camera modes exist: n_chunks > 1, on_chunk or peers return
+ * GSB_ERR_ARGUMENT.  As with camera gradients, those protocols cover the per-gaussian gradient rows of GsbGrads only:
+ * dL_dfeatures is neither handed out chunk by chunk nor added into the owner ranks' buffers. */
+int32_t gsb_backward_batch_features(int32_t V, const GsbSettings *settings, const GsbInputs *in, const GsbState *states,
+                                    const float *out_color, const float *out_invdepth, const float *dL_dcolor,
+                                    const float *dL_dinvdepth, const float *dL_dalpha, const GsbGrads *grads,
+                                    const GsbCameraGrads *cam_grads, const GsbFeatures *features, const GsbPeerTable *peers,
+                                    int32_t accumulate, int32_t n_chunks, gsb_chunk_fn on_chunk, void *chunk_ctx,
+                                    gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream);
+
 /* Lets kernels launched on the CURRENT device dereference pointers into `peer_device`'s memory (cudaDeviceEnablePeerAccess;
  * already-enabled is not an error).  Needed once per peer before gsb_backward_batch_peer is given peer-mapped buffers. */
 int32_t gsb_enable_peer_access(int32_t peer_device);
