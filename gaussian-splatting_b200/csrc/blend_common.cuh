@@ -68,6 +68,37 @@ __device__ __forceinline__ float reduce2_transposed(const float v0, const float 
     return r;
 }
 
+// Lane roles of reduce10_transposed: bits 4, 3, 2 and 1 of the lane id, from lane_mask = 1 << lane.  Each role is then ONE
+// test of one register against a constant (a kernel keeps lane_mask opaque in a register, so a loop does not rebuild it
+// from the lane id; there are not enough predicate registers to keep all four roles resident).
+struct LaneBits {
+    bool b4, b3, b2, b1;
+};
+__device__ __forceinline__ LaneBits lane_bits(const uint32_t lane_mask) {
+    return LaneBits{(lane_mask & 0xffff0000u) != 0u, (lane_mask & 0xff00ff00u) != 0u, (lane_mask & 0xf0f0f0f0u) != 0u,
+                    (lane_mask & 0xccccccccu) != 0u};
+}
+
+// Warp totals of ten per-lane sums v[0..9] (nine with TEN = false: v[9] is not read) in 12 shuffles (5 + 3 + 2 + 1 + 1).
+// Lane L ends with the total of sum  (L & 2) ? 4 + 5 b4 : 2 b2 + b3 + 5 b4  (bK = bit K of L), so lanes
+// 0, 8, 4, 12, 2, 16, 24, 20, 28, 18 hold sums 0..9.  Without v[9], the lanes that would hold it hold sum 4 as well.
+template <bool TEN>
+__device__ __forceinline__ float reduce10_transposed(const float (&v)[10], const LaneBits &L) {
+    float k[5];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) k[i] = (L.b4 ? v[i + 5] : v[i]) + __shfl_xor_sync(0xffffffffu, L.b4 ? v[i] : v[i + 5], 16);
+    if (TEN) k[4] = (L.b4 ? v[9] : v[4]) + __shfl_xor_sync(0xffffffffu, L.b4 ? v[4] : v[9], 16);
+    else     k[4] = v[4] + __shfl_xor_sync(0xffffffffu, v[4], 16);
+    const float m0 = (L.b3 ? k[1] : k[0]) + __shfl_xor_sync(0xffffffffu, L.b3 ? k[0] : k[1], 8);
+    const float m1 = (L.b3 ? k[3] : k[2]) + __shfl_xor_sync(0xffffffffu, L.b3 ? k[2] : k[3], 8);
+    const float m2 = k[4] + __shfl_xor_sync(0xffffffffu, k[4], 8);
+    const float n0 = (L.b2 ? m1 : m0) + __shfl_xor_sync(0xffffffffu, L.b2 ? m0 : m1, 4);
+    const float n1 = m2 + __shfl_xor_sync(0xffffffffu, m2, 4);
+    float r = (L.b1 ? n1 : n0) + __shfl_xor_sync(0xffffffffu, L.b1 ? n0 : n1, 2);
+    r += __shfl_xor_sync(0xffffffffu, r, 1);
+    return r;
+}
+
 // ---- FP32 pairs: two pixels (or two coordinates) carried as one 64-bit register pair ----
 // sm_90 has no packed FP32 instruction, so every pair operation is two scalar round-to-nearest instructions (the _rn
 // intrinsics also keep the compiler from contracting a multiply and an add into an FMA, which would change the bits

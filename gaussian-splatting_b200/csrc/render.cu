@@ -16,9 +16,9 @@
 //
 // Backward (render_bwd_kernel): 2x2 pixels per thread (a warp owns a 16x8 band), so the shared-memory reads, loop
 // overhead and the cross-lane reduction of the ten per-gaussian gradient terms are paid once per four pixels; the
-// two pixels of a row share every per-gaussian operand and are carried as f32x2 register pairs.  The pass walks
-// FRONT to back with two scalars of state per pixel (T and the running dL-weighted front colour F) instead of the
-// ten the back-to-front recursion carries:
+// four pixels are plain scalars (sm_90 has no packed FP32 arithmetic).  The pass walks FRONT to back with two scalars
+// of state per pixel (T and U = S - F, F the running dL-weighted front colour) instead of the ten the back-to-front
+// recursion carries:
 //     dL/dalpha_k = T_k g_k - (S - F_k) / (1 - alpha_k),   g_k = dLdC . c_k + dLdD / z_k,
 //     S = dLdC . C_out + dLdD D_out,   F_k = sum_{j<=k} alpha_j T_j g_j
 // (algebraically the recursion of oracle/gs_oracle.c; background enters through C_out).  The geometric gradient
@@ -168,20 +168,29 @@ render_fwd_kernel(const RenderFwdArgs a) {
     }
 }
 
-// *(float *)(base + off) += v (relaxed, device scope, no return value) for the lanes with off >= 0, as ONE predicated instruction
-__device__ __forceinline__ void red_add_if(char *base, const int off, const float v) {
+// *p += v (relaxed, device scope, no return value) on the lanes with `on`, as ONE predicated instruction
+__device__ __forceinline__ void red_add_on(float *p, const bool on, const float v) {
 #ifdef GSB_HOST_EMUL
-    if (off >= 0) atomicAdd(reinterpret_cast<float *>(base + off), v);
+    if (on) atomicAdd(p, v);
 #else
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ge.s32 p, %1, 0;\n\t@p red.global.add.f32 [%0], %2;\n\t}"
-                 ::"l"(base + (off < 0 ? 0 : off)), "r"(off), "f"(v) : "memory");
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\t@p red.global.add.f32 [%0], %2;\n\t}"
+                 ::"l"(p), "r"((uint32_t)on), "f"(v) : "memory");
 #endif
 }
 
-// Backward.  Arithmetic per lane is IEEE round-to-nearest (the f32x2 helpers are pairs of _rn scalar instructions).
+// Backward.  Scalar IEEE round-to-nearest arithmetic (sm_90 has no packed FP32 instruction, so pairs would buy nothing).
+// Per list entry a lane evaluates its four pixels with the forward kernel's operations, then, if any lane of the warp
+// blends the gaussian:
+//   * U = S - F is carried instead of F, so dL/dalpha = T g - U / (1 - alpha) is one multiply and one FMA on the reciprocal;
+//   * the five raw moments are formed once per lane from four basis sums of G dL/dalpha (all four pixels, column 1, row 1,
+//     pixel (1, 1)): with dx0 = x - px0, sum t dx = dx0 s - s_c, sum t dx^2 = dx0 sum t dx - dx1 s_c, and alike for y and xy;
+//   * they are multiplied by the opacity once, after the reduction (t = o G dL/dalpha is linear in o), on the lanes that
+//     hold them;
+//   * ONE transposed shuffle network (12 shuffles) reduces the nine or ten sums, whose lanes add them to the accumulator row
+//     with one predicated reduction instruction.
 // ALPHA: the rendered alpha A = 1 - final_T is one more channel whose per-gaussian "colour" is 1 and whose background is 0:
 // g_k += dL/dA and S += dL/dA * A.  Then T_k - (A - F_k) / (1 - alpha_k) = T_final / (1 - alpha_k) = dA/dalpha_k, as it must.
-// It has no colour gradient, so the accumulator row, the shuffle networks and the reduction are those of the plain kernel.
+// It has no colour gradient, so the accumulator row and the reduction are those of the plain kernel.
 template <bool DEPTH, bool ALPHA, int MINB>
 __global__ void __launch_bounds__(64, MINB)
 render_bwd_kernel(const RenderBwdArgs a) {
@@ -200,39 +209,35 @@ render_bwd_kernel(const RenderBwdArgs a) {
     // accumulator rows are addressed as (view * P + gaussian) from the batch's base: the per-view offset goes into the staged
     // record once per 128 entries instead of being rebuilt in the loop (five uniform-pipe instructions per iteration before)
     const uint32_t row0 = (uint32_t)(v * (a.sv_dacc / DACC_STRIDE));
-    const uint32_t want = 0xfu << (4 * (threadIdx.x >> 5));
     const int tile = a.tile_order ? (int)a.tile_order[v * a.sv_ranges + blockIdx.x] : (int)blockIdx.x;
     const int ox = (tile % a.gx) * TILE, oy = (tile / a.gx) * TILE;
+    const float fox = (float)ox, foy = (float)oy;
     const int t = threadIdx.x;
     const int px0 = ox + 2 * (t & 7), py0 = oy + 2 * (t >> 3);
-    const float fx0 = (float)px0, fy0 = (float)py0;
     const uint2 range = ranges[tile];
     const size_t HW = (size_t)a.W * a.H;
 
-    // per-pixel state, packed by row: element c of row r is pixel (px0 + c, py0 + r)
-    f32x2 T[2], F[2], S[2], dL0[2], dL1[2], dL2[2], dLd[2], dLa[2];
-    uint32_t last[4];
+    // per-pixel state: pixel i = 2 r + c is (px0 + c, py0 + r).  U = S - F (see above); rem = n_contrib - base, so that the
+    // pixel blends list entry j of the current round (position base + j + 1) iff j < rem.
+    float T[4], U[4], dL0[4], dL1[4], dL2[4], dLd[4], dLa[4];
+    int rem[4];
     uint32_t my_max = 0;
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        float vS[2] = {0.f, 0.f}, v0[2] = {0.f, 0.f}, v1[2] = {0.f, 0.f}, v2[2] = {0.f, 0.f}, vd[2] = {0.f, 0.f}, va[2] = {0.f, 0.f};
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-            const int px = px0 + c, py = py0 + r;
-            last[2 * r + c] = 0u;
-            if (px < a.W && py < a.H) {
-                const size_t pid = (size_t)py * a.W + px;
-                last[2 * r + c] = n_contrib[pid];
-                v0[c] = dL_dcolor[pid]; v1[c] = dL_dcolor[HW + pid]; v2[c] = dL_dcolor[2 * HW + pid];
-                vS[c] = v0[c] * out_color[pid] + v1[c] * out_color[HW + pid] + v2[c] * out_color[2 * HW + pid];
-                if (DEPTH) { vd[c] = a.dL_dinvdepth[v * a.sv_depth + pid]; vS[c] += vd[c] * a.out_invdepth[v * a.sv_depth + pid]; }
-                if (ALPHA) { va[c] = a.dL_dalpha[v * a.sv_depth + pid]; vS[c] += va[c] * (1.0f - a.final_T[v * a.sv_image + pid]); }
-            }
-            my_max = max(my_max, last[2 * r + c]);
+    for (int i = 0; i < 4; ++i) {
+        const int px = px0 + (i & 1), py = py0 + (i >> 1);
+        uint32_t last = 0u;
+        float vS = 0.f, v0 = 0.f, v1 = 0.f, v2 = 0.f, vd = 0.f, va = 0.f;
+        if (px < a.W && py < a.H) {
+            const size_t pid = (size_t)py * a.W + px;
+            last = n_contrib[pid];
+            v0 = dL_dcolor[pid]; v1 = dL_dcolor[HW + pid]; v2 = dL_dcolor[2 * HW + pid];
+            vS = v0 * out_color[pid] + v1 * out_color[HW + pid] + v2 * out_color[2 * HW + pid];
+            if (DEPTH) { vd = a.dL_dinvdepth[v * a.sv_depth + pid]; vS += vd * a.out_invdepth[v * a.sv_depth + pid]; }
+            if (ALPHA) { va = a.dL_dalpha[v * a.sv_depth + pid]; vS += va * (1.0f - a.final_T[v * a.sv_image + pid]); }
         }
-        T[r] = pk1(1.0f); F[r] = pk1(0.0f); S[r] = pk(vS[0], vS[1]);
-        dL0[r] = pk(v0[0], v0[1]); dL1[r] = pk(v1[0], v1[1]); dL2[r] = pk(v2[0], v2[1]); dLd[r] = pk(vd[0], vd[1]);
-        dLa[r] = pk(va[0], va[1]);
+        my_max = max(my_max, last);
+        T[i] = 1.0f; U[i] = vS; dL0[i] = v0; dL1[i] = v1; dL2[i] = v2; dLd[i] = vd; dLa[i] = va;
+        rem[i] = (int)last;
     }
     if (t == 0) s_max = 0;
     __syncthreads();
@@ -241,12 +246,9 @@ render_bwd_kernel(const RenderBwdArgs a) {
     __syncthreads();
     const int todo = (int)s_max;
     const int my_todo = (int)my_max;
-    const f32x2 one2 = pk1(1.0f);
-    const int lane = t & 31;
-    int red_off = (lane & 3) == 0 ? 4 * (lane >> 2) : (lane == 1 ? 32 : (DEPTH && lane == 17 ? 36 : -1));
-#ifndef GSB_HOST_EMUL
-    asm volatile("" : "+r"(red_off));      // opaque from here on: kept in a register instead of being rebuilt from the lane id in the loop
-#endif
+    // After reduce10_transposed a lane holds sum `slot` (= its float slot in the accumulator row); one lane per sum adds it:
+    // lanes 0, 8, 4, 12, 2, 16, 24, 20, 28 (and 18 with the depth sum), i.e. the bits of ADDS.
+    constexpr uint32_t ADDS = DEPTH ? 0x11151115u : 0x11111115u;
 
     for (int base = 0; base < todo; base += MP_R) {
         __syncthreads();
@@ -255,104 +257,88 @@ render_bwd_kernel(const RenderBwdArgs a) {
             const uint32_t g = point_list[range.x + base + k];
             const float4 *rec = splat + (size_t)g * SPLAT_F4;
             const float4 q0 = __ldg(rec), q1 = __ldg(rec + 1), q2 = __ldg(rec + 2);
-            smask[k] = (uint8_t)patch_mask(q0.x, q0.y, q0.z, q0.w, q1.x, q2.z, (float)ox, (float)oy);
+            smask[k] = (uint8_t)patch_mask(q0.x, q0.y, q0.z, q0.w, q1.x, q2.z, fox, foy);
             stage_record(srec[k], q0, q1, q2, row0 + g);
         }
         __syncthreads();
+        // The loop's per-thread constants are formed here, once per round, from an opaque copy of the thread index: hoisted
+        // out of the round loop they would be live across the staging above, which then spills.  Inside the loop they are
+        // neither rebuilt nor recomputed: the pixel coordinates, the lane's address in accumulator row 0 (the loop adds
+        // row * 48 bytes) and lane_mask = 1 << lane, of which every lane role is one test.
+        int tr = t;
+#ifndef GSB_HOST_EMUL
+        asm volatile("" : "+r"(tr));
+#endif
+        const int lane = tr & 31;
+        const int slot = (lane & 2) ? 4 + 5 * (lane >> 4) : ((lane >> 1) & 2) + ((lane >> 3) & 1) + 5 * (lane >> 4);
+        float *dacc_lane = a.dacc + slot;
+        uint32_t lane_mask = 1u << lane;
+#ifndef GSB_HOST_EMUL
+        asm volatile("" : "+l"(dacc_lane), "+r"(lane_mask));
+#endif
+        const float fx0 = fox + (float)(2 * (tr & 7)), fy0 = foy + (float)(2 * (tr >> 3));    // exact: px0, py0
+        const float fx1 = __fadd_rn(fx0, 1.0f), fy1 = __fadd_rn(fy0, 1.0f);
         const int nw = max(0, min(n, my_todo - base));
-        const int cnt = compact_hits(smask, nw, want, slist[t >> 5]);
+        const int cnt = compact_hits(smask, nw, 0xfu << (4 * (tr >> 5)), slist[tr >> 5]);
         for (int kk = 0; kk < cnt; ++kk) {
             const int j = (int)slist[t >> 5][kk];
             const StagedRec &rec = srec[j];
-            const float4 q1 = rec.q1;
-            float4 q0;                                   // {x, y, A', C'}
-            unpk((f32x2)rec.w0.x, q0.x, q0.y);
-            unpk((f32x2)rec.w0.y, q0.z, q0.w);
-            const uint32_t pos = (uint32_t)(base + j + 1);
-            // column-packed terms (shared by both rows): dx, A' dx^2, B' dx
-            const f32x2 dx2 = pk(q0.x - fx0, q0.x - (fx0 + 1.0f));   // same rounding as the forward kernel
-            const f32x2 Axx2 = mul2(mul2(pk1(q0.z), dx2), dx2);
-            const f32x2 Bx2 = mul2(pk1(q1.x), dx2);
-            float dy[2], Cyy[2];
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                dy[r] = q0.y - (fy0 + (float)r);
-                Cyy[r] = __fmul_rn(__fmul_rn(q0.w, dy[r]), dy[r]);
-            }
+            const float4 q1 = rec.q1;                    // {B', o, r, g}
+            float x, y, A, C;                            // A', C'
+            unpk((f32x2)rec.w0.x, x, y);
+            unpk((f32x2)rec.w0.y, A, C);
+            // the forward kernel's operations (x - px == x + (-px)), so that both passes agree bit for bit on alpha
+            const float dx[2] = {__fsub_rn(x, fx0), __fsub_rn(x, fx1)}, dy[2] = {__fsub_rn(y, fy0), __fsub_rn(y, fy1)};
             float G[4], al[4];
             bool valid[4];
             bool any = false;
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                // power2_at(Axx, Cyy, Bx, dy) = fma(Bx, dy, Axx + Cyy), both columns at once
-                const f32x2 p2 = fma2(Bx2, pk1(dy[r]), add2(Axx2, pk1(Cyy[r])));
-                float p[2];
-                unpk(p2, p[0], p[1]);
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const int i = 2 * r + c;
-                    G[i] = ex2_approx(p[c]);
-                    al[i] = fminf(ALPHA_MAX, __fmul_rn(q1.y, G[i]));
-                    valid[i] = (p[c] <= 0.0f) && (al[i] >= ALPHA_MIN) && (pos <= last[i]);
-                    any = any || valid[i];
-                }
+            for (int i = 0; i < 4; ++i) {
+                const float dxc = dx[i & 1], dyr = dy[i >> 1];
+                const float p = power2_at(__fmul_rn(__fmul_rn(A, dxc), dxc), __fmul_rn(__fmul_rn(C, dyr), dyr), __fmul_rn(q1.x, dxc), dyr);
+                G[i] = ex2_approx(p);
+                al[i] = fminf(ALPHA_MAX, __fmul_rn(q1.y, G[i]));
+                valid[i] = (p <= 0.0f) && (al[i] >= ALPHA_MIN) && (j < rem[i]);
+                any = any || valid[i];
             }
             if (!__any_sync(0xffffffffu, any)) continue;
-            const float2 q2 = make_float2(rec.b, rec.inv_z);
-            f32x2 m_x = pk1(0.f), m_y = m_x, m_xx = m_x, m_xy = m_x, m_yy = m_x, g_o = m_x, g_r = m_x, g_g = m_x, g_b = m_x, g_d = m_x;
-            const f32x2 cr = pk1(q1.z), cg = pk1(q1.w), cb = pk1(q2.x), cd = pk1(q2.y), op2 = pk1(q1.y);
+            const float cb = rec.b, cd = rec.inv_z;
+            float Gd[4], sum[10];                        // sum: the accumulator row's slots 0..9 (moments still without o)
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const int i0 = 2 * r, i1 = 2 * r + 1;
-                // invalid lanes: alpha = 0 and G = 0 make every contribution below exactly zero
-                const f32x2 ai = pk(valid[i0] ? al[i0] : 0.0f, valid[i1] ? al[i1] : 0.0f);
-                const f32x2 Gm = pk(valid[i0] ? G[i0] : 0.0f, valid[i1] ? G[i1] : 0.0f);
-                const f32x2 w = mul2(ai, T[r]);
-                f32x2 g = fma2(dL2[r], cb, fma2(dL1[r], cg, mul2(dL0[r], cr)));
-                if (DEPTH) g = fma2(dLd[r], cd, g);
-                if (ALPHA) g = add2(g, dLa[r]);
-                F[r] = fma2(w, g, F[r]);
-                if (r == 0) {
-                    g_r = mul2(w, dL0[r]); g_g = mul2(w, dL1[r]); g_b = mul2(w, dL2[r]);
-                    if (DEPTH) g_d = mul2(w, dLd[r]);
+            for (int i = 0; i < 4; ++i) {
+                // invalid pixels: alpha = 0 and G = 0 make every contribution below exactly zero
+                const float ai = valid[i] ? al[i] : 0.0f, Gi = valid[i] ? G[i] : 0.0f;
+                const float w = __fmul_rn(ai, T[i]);
+                float g = __fmaf_rn(dL2[i], cb, __fmaf_rn(dL1[i], q1.w, __fmul_rn(dL0[i], q1.z)));
+                if (DEPTH) g = __fmaf_rn(dLd[i], cd, g);
+                if (ALPHA) g = __fadd_rn(g, dLa[i]);
+                U[i] = __fmaf_rn(-w, g, U[i]);
+                const float om = __fsub_rn(1.0f, ai);
+                Gd[i] = __fmul_rn(Gi, __fmaf_rn(-U[i], rcp_approx(om), __fmul_rn(T[i], g)));     // G dL/dalpha
+                T[i] = __fmul_rn(T[i], om);
+                if (i == 0) {     // the sums START at the first pixel's terms (0 + x is not folded away: it turns -0 into +0)
+                    sum[6] = __fmul_rn(w, dL0[i]); sum[7] = __fmul_rn(w, dL1[i]); sum[8] = __fmul_rn(w, dL2[i]);
+                    sum[9] = DEPTH ? __fmul_rn(w, dLd[i]) : 0.0f;
                 } else {
-                    g_r = fma2(w, dL0[r], g_r); g_g = fma2(w, dL1[r], g_g); g_b = fma2(w, dL2[r], g_b);
-                    if (DEPTH) g_d = fma2(w, dLd[r], g_d);
-                }
-                const f32x2 om = sub2(one2, ai);
-                float om0, om1;
-                unpk(om, om0, om1);
-                const f32x2 rcp = pk(rcp_approx(om0), rcp_approx(om1));
-                // dL/dalpha = T g - (S - F) / (1 - alpha); multiplied by G (0 for invalid lanes) wherever it is used
-                const f32x2 dLda = sub2(mul2(T[r], g), mul2(sub2(S[r], F[r]), rcp));
-                T[r] = mul2(T[r], om);
-                const f32x2 Gd = mul2(Gm, dLda);
-                const f32x2 tt = mul2(op2, Gd);
-                const f32x2 dy2 = pk1(dy[r]);
-                const f32x2 u = mul2(tt, dx2), vv = mul2(tt, dy2);
-                if (r == 0) {     // the sums START at the first row's terms (0 + x is not folded away: it turns -0 into +0)
-                    g_o = Gd; m_x = u; m_y = vv;
-                    m_xx = mul2(u, dx2); m_xy = mul2(u, dy2); m_yy = mul2(vv, dy2);
-                } else {
-                    g_o = add2(g_o, Gd); m_x = add2(m_x, u); m_y = add2(m_y, vv);
-                    m_xx = fma2(u, dx2, m_xx); m_xy = fma2(u, dy2, m_xy); m_yy = fma2(vv, dy2, m_yy);
+                    sum[6] = __fmaf_rn(w, dL0[i], sum[6]); sum[7] = __fmaf_rn(w, dL1[i], sum[7]); sum[8] = __fmaf_rn(w, dL2[i], sum[8]);
+                    if (DEPTH) sum[9] = __fmaf_rn(w, dLd[i], sum[9]);
                 }
             }
-            // both shuffle networks are issued before the atomic so that their (independent) chains overlap
-            const float ra = reduce8_transposed(hsum(m_x), hsum(m_y), hsum(m_xx), hsum(m_xy), hsum(m_yy), hsum(g_o), hsum(g_r), hsum(g_g));
-            float rb;
-            if (DEPTH) {
-                rb = reduce2_transposed(hsum(g_b), hsum(g_d));
-            } else {
-                rb = hsum(g_b);
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) rb += __shfl_xor_sync(0xffffffffu, rb, o);
-            }
-            // ONE predicated reduction instruction for the ten sums: lanes 0, 4, ..., 28 hold sums 0..7 (ra), lane 1 (and 17 with a
-            // depth gradient) the remaining ones (rb); red_off is the lane's byte offset into the 48-byte accumulator row or -1
-            // (computed once per thread: the loop used to rebuild the lane roles and branch around two atomics every iteration).
-            red_add_if(reinterpret_cast<char *>(a.dacc + (size_t)rec.row * DACC_STRIDE), red_off, red_off >= 32 ? rb : ra);
+            // basis sums over the pixels of column 1 and of row 1; sum 5 (opacity) is the sum over all four
+            const float s_c = __fadd_rn(Gd[1], Gd[3]), s_r = __fadd_rn(Gd[2], Gd[3]);
+            sum[5] = __fadd_rn(__fadd_rn(Gd[0], Gd[2]), s_c);
+            sum[0] = __fmaf_rn(dx[0], sum[5], -s_c);                                   // sum G dL/dalpha dx
+            sum[1] = __fmaf_rn(dy[0], sum[5], -s_r);                                   // ... dy
+            sum[2] = __fmaf_rn(dx[0], sum[0], -__fmul_rn(dx[1], s_c));                 // ... dx^2
+            sum[3] = __fmaf_rn(dy[0], sum[0], __fmaf_rn(-dx[0], s_r, Gd[3]));          // ... dx dy
+            sum[4] = __fmaf_rn(dy[0], sum[1], -__fmul_rn(dy[1], s_r));                 // ... dy^2
+            const LaneBits lb = lane_bits(lane_mask);
+            float r = reduce10_transposed<DEPTH>(sum, lb);
+            r = lb.b4 ? r : __fmul_rn(r, q1.y);          // lanes 0..15 hold sums 0..4: the moments' opacity factor
+            red_add_on(dacc_lane + (size_t)rec.row * DACC_STRIDE, (lane_mask & ADDS) != 0u, r);
         }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) rem[i] -= MP_R;
     }
 }
 
