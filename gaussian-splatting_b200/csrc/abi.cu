@@ -264,11 +264,11 @@ static int forward_impl(const char *fn, const GsbSettings *s, const GsbInputs *i
     if (!st->image) return GSB_ERR_ALLOC;
     carve_image(st->image, npix, iv);
 
-    uint32_t *key, *idx, *key_alt, *idx_alt, *tiles, *offsets, *partials; uint2 *rect; unsigned long long *total; char *sortscr;
+    uint32_t *key, *idx, *key_alt, *idx_alt, *tiles, *offsets; uint2 *rect; unsigned long long *scan_state, *total; char *sortscr;
     auto carve0 = [&](Carver &c) {
         key = c.take<uint32_t>(Pn); idx = c.take<uint32_t>(Pn); key_alt = c.take<uint32_t>(Pn); idx_alt = c.take<uint32_t>(Pn);
         tiles = c.take<uint32_t>(Pn); rect = c.take<uint2>(Pn); offsets = c.take<uint32_t>(Pn);
-        partials = c.take<uint32_t>(scan_partials_count(P)); total = c.take<unsigned long long>(4);
+        scan_state = c.take<unsigned long long>(scan_state_count(P)); total = c.take<unsigned long long>(4);
         sortscr = c.take<char>(sort_scratch_bytes(P));
     };
     Carver c0(nullptr);
@@ -280,8 +280,8 @@ static int forward_impl(const char *fn, const GsbSettings *s, const GsbInputs *i
 
     BinArgs ba;
     ba.P = P; ba.num_tiles = num_tiles; ba.gx = cam.gx; ba.order = idx; ba.tiles = tiles; ba.rect = rect; ba.splat = splat;
-    ba.offsets = offsets; ba.partials = partials; ba.total = total;
-    ba.sv_gauss = 0; ba.sv_splat = 0; ba.sv_partials = 0; ba.sv_inst = 0;
+    ba.offsets = offsets; ba.scan_state = scan_state; ba.total = total;
+    ba.sv_gauss = 0; ba.sv_splat = 0; ba.sv_scan = 0; ba.sv_inst = 0;
     st->splat = splat; st->final_T = iv.final_T; st->n_contrib = iv.n_contrib;
 
     // binning + blend for an instance capacity `cap`; the true count is read by the kernels from *n_dev when given
@@ -303,9 +303,13 @@ static int forward_impl(const char *fn, const GsbSettings *s, const GsbInputs *i
             Carver c1r(scr1);
             uint32_t *inst_tile = c1r.take<uint32_t>(Dn), *inst_tile_alt = c1r.take<uint32_t>(Dn), *inst_gauss_alt = c1r.take<uint32_t>(Dn);
             char *sortscr1 = c1r.take<char>(sort_scratch_bytes(cap));
-            r = launch_emit(ba, 1, inst_tile, bv.point_list, cap, debug, stream);
+            SortDigits dg;
+            r = sort_prepare(cap, 1, 0, tile_bits, sortscr1, stream, &dg);
             if (r) return r;
-            r = sort_pairs(inst_tile, bv.point_list, inst_tile_alt, inst_gauss_alt, cap, n_dev, 0, tile_bits, sortscr1, debug, stream, 1, 0);
+            r = launch_emit(ba, 1, inst_tile, bv.point_list, cap, dg, debug, stream);
+            if (r) return r;
+            r = sort_pairs(inst_tile, bv.point_list, inst_tile_alt, inst_gauss_alt, cap, n_dev, 0, tile_bits, sortscr1, debug, stream, 1, 0,
+                           true);
             if (r) return r;
             r = launch_tile_ranges(inst_tile, cap, n_dev, num_tiles, bv.ranges, 1, 0, debug, stream);
             if (r) return r;
@@ -690,12 +694,12 @@ static int forward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs *
     }
 
     // ---- per-gaussian scratch, [V][Pn] ----
-    const size_t np = scan_partials_count(P);
-    uint32_t *key, *idx, *key_alt, *idx_alt, *tiles, *offsets, *partials; uint2 *rect; unsigned long long *total; char *sortscr;
+    const size_t np = scan_state_count(P);
+    uint32_t *key, *idx, *key_alt, *idx_alt, *tiles, *offsets; uint2 *rect; unsigned long long *scan_state, *total; char *sortscr;
     auto carve0 = [&](Carver &c) {
         key = c.take<uint32_t>(V * Pn); idx = c.take<uint32_t>(V * Pn); key_alt = c.take<uint32_t>(V * Pn); idx_alt = c.take<uint32_t>(V * Pn);
         tiles = c.take<uint32_t>(V * Pn); rect = c.take<uint2>(V * Pn); offsets = c.take<uint32_t>(V * Pn);
-        partials = c.take<uint32_t>(V * np); total = c.take<unsigned long long>(GSB_MAX_VIEWS);
+        scan_state = c.take<unsigned long long>(V * np); total = c.take<unsigned long long>(GSB_MAX_VIEWS);
         sortscr = c.take<char>(sort_scratch_bytes(P, V));
     };
     Carver c0n(nullptr);
@@ -719,8 +723,8 @@ static int forward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs *
     if (rc) return rc;
     BinArgs ba;
     ba.P = P; ba.num_tiles = num_tiles; ba.gx = c0.gx; ba.order = idx; ba.tiles = tiles; ba.rect = rect; ba.splat = splat;
-    ba.offsets = offsets; ba.partials = partials; ba.total = total;
-    ba.sv_gauss = Pn; ba.sv_splat = sv_splat; ba.sv_partials = np; ba.sv_inst = 0;
+    ba.offsets = offsets; ba.scan_state = scan_state; ba.total = total;
+    ba.sv_gauss = Pn; ba.sv_splat = sv_splat; ba.sv_scan = np; ba.sv_inst = 0;
     rc = launch_tile_scan(ba, V, debug, stream);
     if (rc) return rc;
     unsigned long long *h = nullptr;
@@ -764,9 +768,13 @@ static int forward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs *
             char *sortscr1 = c1r.take<char>(sort_scratch_bytes(cap, V));
             BinArgs bb = ba;
             bb.sv_inst = capn;
-            r = launch_emit(bb, V, inst_tile, point_list, cap, debug, stream);
+            SortDigits dg;
+            r = sort_prepare(cap, V, 0, tile_bits, sortscr1, stream, &dg);
             if (r) return r;
-            r = sort_pairs(inst_tile, point_list, inst_tile_alt, inst_gauss_alt, cap, total, 0, tile_bits, sortscr1, debug, stream, V, capn);
+            r = launch_emit(bb, V, inst_tile, point_list, cap, dg, debug, stream);
+            if (r) return r;
+            r = sort_pairs(inst_tile, point_list, inst_tile_alt, inst_gauss_alt, cap, total, 0, tile_bits, sortscr1, debug, stream, V, capn,
+                           true);
             if (r) return r;
             r = launch_tile_ranges(inst_tile, cap, total, num_tiles, ranges, V, capn, debug, stream);
             if (r) return r;

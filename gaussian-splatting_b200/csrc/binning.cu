@@ -1,5 +1,5 @@
-// binning.cu -- tile binning: scan of tiles-touched in depth order (K2), instance emission (K3) and
-// per-tile ranges of the tile-sorted instance list (K5).
+// binning.cu -- tile binning: scan of tiles-touched in depth order (K2), instance emission with the tile sort's digit
+// histograms (K3) and per-tile ranges of the tile-sorted instance list (K5).
 //
 // Replaces the cub::DeviceScan::InclusiveSum call, duplicateWithKeys and identifyTileRanges of the
 // reference's cuda_rasterizer/rasterizer_impl.cu (named in BASELINE.json north_star; absent from
@@ -15,7 +15,8 @@ constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_IPT = 8;
 constexpr int SCAN_CHUNK = SCAN_THREADS * SCAN_IPT;
 
-size_t scan_partials_count(int P) { return (size_t)ceil_div(P > 0 ? P : 1, SCAN_CHUNK) + 1; }
+// per view: a ticket counter, then one status word per chunk (decoupled look-back)
+size_t scan_state_count(int P) { return (size_t)ceil_div(P > 0 ? P : 1, SCAN_CHUNK) + 1; }
 
 __device__ __forceinline__ uint32_t block_exclusive_scan_256(const uint32_t v, uint32_t *warp_sums, uint32_t &block_total) {
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -39,50 +40,26 @@ __device__ __forceinline__ uint32_t block_exclusive_scan_256(const uint32_t v, u
     return prefix + incl - v;
 }
 
-__global__ void __launch_bounds__(SCAN_THREADS)
-scan_reduce_kernel(BinArgs a) {
-    __shared__ uint32_t warp_sums[SCAN_THREADS / 32];
-    a.order += blockIdx.y * a.sv_gauss; a.tiles += blockIdx.y * a.sv_gauss; a.partials += blockIdx.y * a.sv_partials;
-    const int base = blockIdx.x * SCAN_CHUNK + threadIdx.x * SCAN_IPT;
-    uint32_t s = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_IPT; ++k) {
-        const int r = base + k;
-        if (r < a.P) s += a.tiles[a.order[r]];
-    }
-    uint32_t total;
-    block_exclusive_scan_256(s, warp_sums, total);
-    if (threadIdx.x == 0) a.partials[blockIdx.x] = total;
-}
+// status word of a chunk: bits 63..62 = 0 not ready | 1 chunk total | 2 inclusive prefix; bits 61..0 = the sum
+#define SCAN_FLAG_AGG (1ull << 62)
+#define SCAN_FLAG_PREFIX (2ull << 62)
+#define SCAN_VALUE_MASK ((1ull << 62) - 1ull)
 
-// single block: exclusive scan of the per-chunk totals (64-bit running sum), grand total -> *total
+// K2: offsets[r] = sum of tiles[order[r']] over r' < r, in one pass.  Chunks take tickets, so a chunk only waits for chunks
+// that started before it; warp 0 finds the chunk's prefix by walking back over 32 predecessors' status words at a time.
+// The 64-bit running sum gives the exact per-view total (the host rejects totals >= 2^31; offsets are that sum mod 2^32).
 __global__ void __launch_bounds__(SCAN_THREADS)
-scan_partials_kernel(uint32_t *partials, const int n, unsigned long long *total_out, const size_t sv_partials) {
+tile_scan_kernel(BinArgs a) {
     __shared__ uint32_t warp_sums[SCAN_THREADS / 32];
-    partials += blockIdx.y * sv_partials; total_out += blockIdx.y;
-    __shared__ unsigned long long carry_s;
-    if (threadIdx.x == 0) carry_s = 0ull;
+    __shared__ uint32_t s_chunk;
+    __shared__ unsigned long long s_prefix;
+    a.order += blockIdx.y * a.sv_gauss; a.tiles += blockIdx.y * a.sv_gauss; a.offsets += blockIdx.y * a.sv_gauss;
+    unsigned long long *ticket = a.scan_state + blockIdx.y * a.sv_scan;
+    volatile unsigned long long *status = ticket + 1;
+    if (threadIdx.x == 0) s_chunk = (uint32_t)atomicAdd(ticket, 1ull);
     __syncthreads();
-    for (int base = 0; base < n; base += SCAN_THREADS) {
-        const int i = base + threadIdx.x;
-        const uint32_t v = i < n ? partials[i] : 0u;
-        uint32_t total;
-        const uint32_t excl = block_exclusive_scan_256(v, warp_sums, total);
-        const unsigned long long carry = carry_s;
-        if (i < n) partials[i] = (uint32_t)(carry + excl);
-        __syncthreads();
-        if (threadIdx.x == 0) carry_s = carry + total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total_out = carry_s;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS)
-scan_apply_kernel(BinArgs a) {
-    __shared__ uint32_t warp_sums[SCAN_THREADS / 32];
-    a.order += blockIdx.y * a.sv_gauss; a.tiles += blockIdx.y * a.sv_gauss; a.partials += blockIdx.y * a.sv_partials;
-    a.offsets += blockIdx.y * a.sv_gauss;
-    const int base = blockIdx.x * SCAN_CHUNK + threadIdx.x * SCAN_IPT;
+    const uint32_t b = s_chunk;
+    const int base = (int)b * SCAN_CHUNK + threadIdx.x * SCAN_IPT;
     uint32_t v[SCAN_IPT];
     uint32_t s = 0;
 #pragma unroll
@@ -92,7 +69,35 @@ scan_apply_kernel(BinArgs a) {
         s += v[k];
     }
     uint32_t total;
-    uint32_t run = block_exclusive_scan_256(s, warp_sums, total) + a.partials[blockIdx.x];
+    const uint32_t excl = block_exclusive_scan_256(s, warp_sums, total);
+    if (threadIdx.x < 32) {
+        const int lane = threadIdx.x;
+        unsigned long long prefix = 0;
+        if (b == 0) {
+            if (lane == 0) status[0] = SCAN_FLAG_PREFIX | total;
+        } else {
+            if (lane == 0) status[b] = SCAN_FLAG_AGG | total;
+            for (int64_t q = (int64_t)b - 1 - lane;; q -= 32) {
+                unsigned long long w = q >= 0 ? status[q] : SCAN_FLAG_PREFIX;
+                while (!__all_sync(0xffffffffu, (w >> 62) != 0ull))
+                    if ((w >> 62) == 0ull) w = status[q];
+                // the nearest inclusive prefix ends the walk: sum the lanes up to it
+                const uint32_t at_prefix = __ballot_sync(0xffffffffu, (w >> 62) == 2ull);
+                unsigned long long x = (at_prefix == 0u || lane < __ffs(at_prefix)) ? (w & SCAN_VALUE_MASK) : 0ull;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+                prefix += x;
+                if (at_prefix) break;
+            }
+            if (lane == 0) status[b] = SCAN_FLAG_PREFIX | ((prefix + total) & SCAN_VALUE_MASK);
+        }
+        if (lane == 0) {
+            s_prefix = prefix;
+            if (b == gridDim.x - 1) a.total[blockIdx.y] = prefix + total;
+        }
+    }
+    __syncthreads();
+    uint32_t run = (uint32_t)s_prefix + excl;
 #pragma unroll
     for (int k = 0; k < SCAN_IPT; ++k) {
         const int r = base + k;
@@ -103,10 +108,8 @@ scan_apply_kernel(BinArgs a) {
 
 int launch_tile_scan(const BinArgs &a, int V, bool debug, cudaStream_t stream) {
     const int nchunks = (int)ceil_div(a.P, SCAN_CHUNK);
-    GSB_LAUNCH("scan_reduce", debug, stream, scan_reduce_kernel, dim3(nchunks, V), SCAN_THREADS, 0, a);
-    GSB_LAUNCH("scan_partials", debug, stream, scan_partials_kernel, dim3(1, V), SCAN_THREADS, 0, a.partials, nchunks, a.total,
-               a.sv_partials);
-    GSB_LAUNCH("scan_apply", debug, stream, scan_apply_kernel, dim3(nchunks, V), SCAN_THREADS, 0, a);
+    GSB_CUDA(cudaMemsetAsync(a.scan_state, 0, ((size_t)(V - 1) * a.sv_scan + scan_state_count(a.P)) * sizeof(unsigned long long), stream));
+    GSB_LAUNCH("tile_scan", debug, stream, tile_scan_kernel, dim3(nchunks, V), SCAN_THREADS, 0, a);
     return GSB_OK;
 }
 
@@ -121,55 +124,101 @@ int launch_count_max(unsigned long long *counts, int V, bool debug, cudaStream_t
     return GSB_OK;
 }
 
-// K3: one thread per depth rank; writes (tile id, gaussian id) for every tile the gaussian's cull ellipse meets.
-__global__ void __launch_bounds__(256)
-emit_kernel(BinArgs a, uint32_t *__restrict__ inst_tile, uint32_t *__restrict__ inst_gauss, const uint32_t cap) {
+// K3: writes (tile id, gaussian id) for every tile the cull ellipse of a gaussian meets, gaussians in depth order.
+// Each lane walks the tiles of one gaussian (the rows and spans of cull_rows / cull_span, or the whole rectangle when culling
+// is off); the 32 gaussians of a warp are consecutive depth ranks, so their instances form one contiguous slot range, which
+// the warp stages in shared memory a window at a time and stores with consecutive lanes on consecutive slots.  The block also
+// counts the digits of the tile sort's passes (dg) over the slots it wrote, so that sort_pairs needs no histogram kernel.
+constexpr int EMIT_THREADS = 256;
+constexpr int EMIT_WINDOW = 256;   // slots per warp and round
+static_assert(EMIT_THREADS == GSB_SORT_RADIX, "one histogram bin per thread");
+
+__global__ void __launch_bounds__(EMIT_THREADS)
+emit_kernel(BinArgs a, uint32_t *__restrict__ inst_tile, uint32_t *__restrict__ inst_gauss, const uint32_t cap, const SortDigits dg) {
+    __shared__ uint32_t s_tile[EMIT_THREADS / 32][EMIT_WINDOW], s_gauss[EMIT_THREADS / 32][EMIT_WINDOW];
+    __shared__ uint32_t hist[GSB_SORT_MAX_PASSES][GSB_SORT_RADIX];
     a.order += blockIdx.y * a.sv_gauss; a.tiles += blockIdx.y * a.sv_gauss; a.rect += blockIdx.y * a.sv_gauss;
     a.offsets += blockIdx.y * a.sv_gauss; a.splat += blockIdx.y * a.sv_splat;
     inst_tile += blockIdx.y * a.sv_inst; inst_gauss += blockIdx.y * a.sv_inst;
-    const int r = blockIdx.x * 256 + threadIdx.x;
-    if (r >= a.P) return;
-    const uint32_t g = a.order[r];
-    uint32_t n = a.tiles[g];
-    if (n == 0) return;
-    const uint32_t start = a.offsets[r];
-    // speculative capacity (abi.cu): never write past it; the host re-runs binning when the count did not fit
-    if (start >= cap) return;
-    n = min(n, cap - start);
-    const float4 q0 = a.splat[(size_t)g * SPLAT_F4], q1 = a.splat[(size_t)g * SPLAT_F4 + 1], q2 = a.splat[(size_t)g * SPLAT_F4 + 2];
-    const uint2 rc = a.rect[g];
-    CullGeom cg;
-    cg.cx = q0.x; cg.cy = q0.y; cg.A = q0.z; cg.B = q0.w; cg.C = q1.x; cg.lim = q2.z;
-    cg.rx0 = (int)(rc.x & 0xffffu); cg.rx1 = (int)(rc.x >> 16);
-    cg.ry0 = (int)(rc.y & 0xffffu); cg.ry1 = (int)(rc.y >> 16);
-    uint32_t k = 0;
-    if (cg.lim > 1.0e38f) {  // culling disabled: the whole rectangle
-        for (int ty = cg.ry0; ty < cg.ry1; ++ty)
-            for (int tx = cg.rx0; tx < cg.rx1 && k < n; ++tx, ++k) {
-                inst_tile[start + k] = (uint32_t)(ty * a.gx + tx);
-                inst_gauss[start + k] = g;
-            }
-    } else {
-        int ty0, ty1;
-        cull_rows(cg, ty0, ty1);
-        for (int ty = ty0; ty < ty1; ++ty) {
-            int tx0, tx1;
-            cull_span(cg, ty, tx0, tx1);
-            for (int tx = tx0; tx < tx1 && k < n; ++tx, ++k) {
-                inst_tile[start + k] = (uint32_t)(ty * a.gx + tx);
-                inst_gauss[start + k] = g;
-            }
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    for (int p = 0; p < dg.npass; ++p) hist[p][tid] = 0;
+
+    // this lane's gaussian and its slots [start, start + n)
+    const int r = blockIdx.x * EMIT_THREADS + tid;
+    uint32_t g = 0, n = 0, start = 0;
+    if (r < a.P) {
+        g = a.order[r];
+        n = a.tiles[g];
+        if (n) {
+            start = a.offsets[r];
+            // speculative capacity (abi.cu): never write past it; the host re-runs binning when the count did not fit
+            n = start < cap ? min(n, cap - start) : 0u;
         }
     }
-    // never taken when count and emit agree; keeps the slot range well defined if they ever do not
-    for (; k < n; ++k) {
-        inst_tile[start + k] = (uint32_t)a.num_tiles;
-        inst_gauss[start + k] = g;
+    // tile walk: row ty of [ty, ty1), columns [tx, tx1) of that row still to come
+    CullGeom cg;
+    int ty = 0, ty1 = 0, tx = 0, tx1 = 0;
+    bool whole = false;
+    if (n) {
+        const float4 q0 = a.splat[(size_t)g * SPLAT_F4], q1 = a.splat[(size_t)g * SPLAT_F4 + 1], q2 = a.splat[(size_t)g * SPLAT_F4 + 2];
+        const uint2 rc = a.rect[g];
+        cg.cx = q0.x; cg.cy = q0.y; cg.A = q0.z; cg.B = q0.w; cg.C = q1.x; cg.lim = q2.z;
+        cg.rx0 = (int)(rc.x & 0xffffu); cg.rx1 = (int)(rc.x >> 16);
+        cg.ry0 = (int)(rc.y & 0xffffu); cg.ry1 = (int)(rc.y >> 16);
+        whole = cg.lim > 1.0e38f;     // culling disabled: the whole rectangle
+        if (whole) { ty = cg.ry0; ty1 = cg.ry1; } else cull_rows(cg, ty, ty1);
+        ty -= 1;
+        tx = tx1 = 0;
+    }
+    auto advance_row = [&]() {
+        while (tx >= tx1 && ++ty < ty1) {
+            if (whole) { tx = cg.rx0; tx1 = cg.rx1; } else cull_span(cg, ty, tx, tx1);
+        }
+    };
+    if (n) advance_row();
+    __syncthreads();     // histogram zeroed
+
+    const uint32_t active = __ballot_sync(0xffffffffu, n != 0u);
+    if (active) {
+        const int first = __ffs(active) - 1, last = 31 - __clz(active);
+        const uint32_t lo = __shfl_sync(0xffffffffu, start, first), hi = __shfl_sync(0xffffffffu, start + n, last);
+        uint32_t k = 0;
+        for (uint32_t base = lo; base < hi; base += EMIT_WINDOW) {
+            const uint32_t end = min(hi, base + EMIT_WINDOW);
+            for (; k < n && start + k < end; ++k) {
+                uint32_t t = (uint32_t)a.num_tiles;   // past the last tile: never taken when count and emit agree
+                if (ty < ty1) {
+                    t = (uint32_t)(ty * a.gx + tx);
+                    ++tx;
+                    advance_row();
+                }
+                s_tile[w][start + k - base] = t;
+                s_gauss[w][start + k - base] = g;
+            }
+            __syncwarp();
+            for (uint32_t j = lane; j < end - base; j += 32) {
+                const uint32_t t = s_tile[w][j];
+                inst_tile[base + j] = t;
+                inst_gauss[base + j] = s_gauss[w][j];
+#pragma unroll
+                for (int p = 0; p < GSB_SORT_MAX_PASSES; ++p)
+                    if (p < dg.npass) atomicAdd(&hist[p][(t >> dg.shift[p]) & dg.mask[p]], 1u);
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    uint32_t *ghist = dg.ghist + blockIdx.y * (GSB_SORT_MAX_PASSES * GSB_SORT_RADIX);
+    for (int p = 0; p < dg.npass; ++p) {
+        const uint32_t c = hist[p][tid];
+        if (c) atomicAdd(&ghist[p * GSB_SORT_RADIX + tid], c);
     }
 }
 
-int launch_emit(const BinArgs &a, int V, uint32_t *inst_tile, uint32_t *inst_gauss, int64_t cap, bool debug, cudaStream_t stream) {
-    GSB_LAUNCH("emit", debug, stream, emit_kernel, dim3((int)ceil_div(a.P, 256), V), 256, 0, a, inst_tile, inst_gauss, (uint32_t)cap);
+int launch_emit(const BinArgs &a, int V, uint32_t *inst_tile, uint32_t *inst_gauss, int64_t cap, const SortDigits &dg, bool debug,
+                cudaStream_t stream) {
+    GSB_LAUNCH("emit", debug, stream, emit_kernel, dim3((int)ceil_div(a.P, EMIT_THREADS), V), EMIT_THREADS, 0, a, inst_tile, inst_gauss,
+               (uint32_t)cap, dg);
     return GSB_OK;
 }
 

@@ -170,10 +170,21 @@ size_t sort_scratch_bytes(int64_t n, int V = 1);
 // n sizes the launch; if n_dev != NULL the kernels sort min(*n_dev, n) pairs (count known only on the device).
 // V > 1 (view batch): V independent sorts in the same launches; view v's arrays start at base + v * sv elements and
 // n_dev is an array of V counts.
+// hist_ready: the scratch was zeroed and its digit histograms filled by the caller (sort_prepare), so the sort skips both.
 int sort_pairs(uint32_t *keys, uint32_t *vals, uint32_t *keys_alt, uint32_t *vals_alt, int64_t n,
                const unsigned long long *n_dev, int begin_bit, int end_bit, void *scratch, bool debug,
-               cudaStream_t stream, int V = 1, size_t sv = 0);
+               cudaStream_t stream, int V = 1, size_t sv = 0, bool hist_ready = false);
 constexpr int GSB_SORT_MAX_VIEWS = 16, GSB_SORT_MAX_PASSES = 4, GSB_SORT_RADIX = 256;
+// The digits of a sort_pairs call: pass p sorts on (key >> shift[p]) & mask[p].  ghist[view][pass][digit] are the counts of
+// the keys that will be sorted, which a kernel that produces the keys can build (binning.cu emit) instead of sort_pairs.
+struct SortDigits {
+    int npass;
+    int shift[GSB_SORT_MAX_PASSES];
+    uint32_t mask[GSB_SORT_MAX_PASSES];
+    uint32_t *ghist;   // [GSB_SORT_MAX_VIEWS][GSB_SORT_MAX_PASSES][GSB_SORT_RADIX]
+};
+// Zeroes the scratch of a later sort_pairs(..., hist_ready = true) call with the same n, V and bits, and describes its digits.
+int sort_prepare(int64_t n, int V, int begin_bit, int end_bit, void *scratch, cudaStream_t stream, SortDigits *out);
 extern int g_sort_force_small;
 extern int g_pre_tma;
 

@@ -82,14 +82,14 @@ struct BinArgs {
     // view-batch launches (blockIdx.y = view): strides between the views' arrays, in elements; 0 for single view
     size_t sv_gauss;          // order / tiles / rect / offsets
     size_t sv_splat;          // float4
-    size_t sv_partials;
+    size_t sv_scan;           // scan_state
     size_t sv_inst;           // instance arrays (capacity)
     const uint32_t *order;    // [P] gaussian ids in depth order
     const uint32_t *tiles;    // [P]
     const uint2 *rect;        // [P]
     const float4 *splat;
     uint32_t *offsets;        // [P] exclusive scan of tiles in depth order
-    uint32_t *partials;       // scan scratch
+    unsigned long long *scan_state;   // [V][scan_state_count(P)] scan scratch, zeroed by launch_tile_scan
     unsigned long long *total;  // device scalar: D
 };
 
@@ -161,12 +161,14 @@ int launch_preprocess_bwd_batch(const CamArgsBatch &cb, const PreBwdArgs &a, con
 int launch_mark_visible(int P, const float *means, const float *view, uint8_t *present, cudaStream_t stream);
 int launch_camera_grad_reduce(const CamReduceArgs &r, bool accumulate, bool debug, cudaStream_t stream);
 
-size_t scan_partials_count(int P);
+size_t scan_state_count(int P);
 // V > 1: blockIdx.y = view, arrays offset by the BinArgs strides; totals / n_dev are arrays of V counts
 int launch_tile_scan(const BinArgs &a, int V, bool debug, cudaStream_t stream);
 // async forward: counts[GSB_MAX_VIEWS] = max(counts[GSB_MAX_VIEWS], counts[0..V))  (running maximum the host polls later)
 int launch_count_max(unsigned long long *counts, int V, bool debug, cudaStream_t stream);
-int launch_emit(const BinArgs &a, int V, uint32_t *inst_tile, uint32_t *inst_gauss, int64_t cap, bool debug, cudaStream_t stream);
+// also fills dg.ghist, the digit histograms of the tile sort of the emitted keys (sort_prepare before, sort_pairs(hist_ready) after)
+int launch_emit(const BinArgs &a, int V, uint32_t *inst_tile, uint32_t *inst_gauss, int64_t cap, const SortDigits &dg, bool debug,
+                cudaStream_t stream);
 int launch_tile_ranges(const uint32_t *sorted_tiles, int64_t D, const unsigned long long *n_dev, int num_tiles,
                        uint2 *ranges, int V, size_t sv_inst, bool debug, cudaStream_t stream);
 

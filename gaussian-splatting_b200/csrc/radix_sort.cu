@@ -270,13 +270,10 @@ static size_t onesweep_scratch_bytes(int64_t n, int V) {
     return align_up((size_t)GSB_SORT_MAX_VIEWS * OS_MAX_PASSES * RADIX * 4 + 256 + (size_t)V * OS_MAX_PASSES * nblocks * RADIX * 4, 256);
 }
 
-static int onesweep_sort(uint32_t *keys, uint32_t *vals, uint32_t *keys_alt, uint32_t *vals_alt, int64_t n,
-                         const unsigned long long *n_dev, int begin_bit, int end_bit, void *scratch, bool debug,
-                         cudaStream_t stream, int V, size_t sv) {
-    OnesweepPasses ps;
+// the key bits are split EVENLY over the fewest passes (13 tile bits = 7 + 6, not 8 + 5): a pass with fewer digits writes
+// longer runs per digit out of every block
+static int onesweep_passes(int begin_bit, int end_bit, OnesweepPasses &ps) {
     ps.npass = 0;
-    // the key bits are split EVENLY over the fewest passes (13 tile bits = 7 + 6, not 8 + 5): a pass with fewer digits writes
-    // longer runs per digit out of every block
     const int total_bits = end_bit - begin_bit, npass = (total_bits + RADIX_BITS - 1) / RADIX_BITS;
     if (npass > OS_MAX_PASSES) { set_error("onesweep: more than %d passes", OS_MAX_PASSES); return GSB_ERR_ARGUMENT; }
     for (int p = 0, bit = begin_bit; p < npass; ++p) {
@@ -286,17 +283,32 @@ static int onesweep_sort(uint32_t *keys, uint32_t *vals, uint32_t *keys_alt, uin
         bit += bits;
         ++ps.npass;
     }
+    return GSB_OK;
+}
+
+// scratch layout: ghist[16 views][4][256] | ticket[16][4] (256 B) | status[V][npass][nblocks][256]
+static size_t onesweep_zero_bytes(int64_t n, int V, int npass) {
+    const int64_t nblocks = ceil_div(n, SORT_THREADS * sort_ipt(n));
+    return (size_t)GSB_SORT_MAX_VIEWS * OS_MAX_PASSES * RADIX * 4 + 256 + (size_t)V * npass * nblocks * RADIX * 4;
+}
+
+static int onesweep_sort(uint32_t *keys, uint32_t *vals, uint32_t *keys_alt, uint32_t *vals_alt, int64_t n,
+                         const unsigned long long *n_dev, int begin_bit, int end_bit, void *scratch, bool debug,
+                         cudaStream_t stream, int V, size_t sv, bool hist_ready) {
+    OnesweepPasses ps;
+    int rc = onesweep_passes(begin_bit, end_bit, ps);
+    if (rc) return rc;
     const int ipt = sort_ipt(n);
     const int nblocks = (int)ceil_div(n, SORT_THREADS * ipt);
-    // layout: ghist[16 views][4][256] | ticket[16][4] (256 B) | status[V][npass][nblocks][256]
     uint32_t *ghist = static_cast<uint32_t *>(scratch);
     uint32_t *ticket = ghist + GSB_SORT_MAX_VIEWS * OS_MAX_PASSES * RADIX;
     uint32_t *status = ticket + 64;
     const size_t sv_status = (size_t)ps.npass * nblocks * RADIX;
-    const size_t zero_bytes = (size_t)GSB_SORT_MAX_VIEWS * OS_MAX_PASSES * RADIX * 4 + 256 + (size_t)V * sv_status * 4;
-    GSB_CUDA(cudaMemsetAsync(scratch, 0, zero_bytes, stream));
-    const int hist_blocks = (int)(ceil_div(n, 256 * 16) < NUM_SMS * 8 ? ceil_div(n, 256 * 16) : NUM_SMS * 8);
-    GSB_LAUNCH("sort_hist", debug, stream, onesweep_hist_kernel, dim3(hist_blocks, V), 256, 0, keys, ghist, n, n_dev, ps, sv);
+    if (!hist_ready) {
+        GSB_CUDA(cudaMemsetAsync(scratch, 0, onesweep_zero_bytes(n, V, ps.npass), stream));
+        const int hist_blocks = (int)(ceil_div(n, 256 * 16) < NUM_SMS * 8 ? ceil_div(n, 256 * 16) : NUM_SMS * 8);
+        GSB_LAUNCH("sort_hist", debug, stream, onesweep_hist_kernel, dim3(hist_blocks, V), 256, 0, keys, ghist, n, n_dev, ps, sv);
+    }
     uint32_t *kin = keys, *vin = vals, *kout = keys_alt, *vout = vals_alt;
     for (int p = 0; p < ps.npass; ++p) {
         uint32_t *st = status + (size_t)p * nblocks * RADIX;
@@ -315,16 +327,30 @@ static int onesweep_sort(uint32_t *keys, uint32_t *vals, uint32_t *keys_alt, uin
 
 size_t sort_scratch_bytes(int64_t n, int V) { return onesweep_scratch_bytes(n, V); }
 
+int sort_prepare(int64_t n, int V, int begin_bit, int end_bit, void *scratch, cudaStream_t stream, SortDigits *out) {
+    OnesweepPasses ps;
+    int rc = onesweep_passes(begin_bit, end_bit, ps);
+    if (rc) return rc;
+    out->npass = ps.npass;
+    for (int p = 0; p < OS_MAX_PASSES; ++p) {
+        out->shift[p] = p < ps.npass ? ps.shift[p] : 0;
+        out->mask[p] = p < ps.npass ? ps.mask[p] : 0u;
+    }
+    out->ghist = static_cast<uint32_t *>(scratch);
+    if (n > 0) GSB_CUDA(cudaMemsetAsync(scratch, 0, onesweep_zero_bytes(n, V, ps.npass), stream));
+    return GSB_OK;
+}
+
 int sort_pairs(uint32_t *keys, uint32_t *vals, uint32_t *keys_alt, uint32_t *vals_alt, int64_t n,
                const unsigned long long *n_dev, int begin_bit, int end_bit, void *scratch, bool debug,
-               cudaStream_t stream, int V, size_t sv) {
+               cudaStream_t stream, int V, size_t sv, bool hist_ready) {
     if (n <= 0 || end_bit <= begin_bit) return GSB_OK;
     if (n >= (int64_t)1 << 30) {
         set_error("sort_pairs: n=%lld does not fit 30-bit positions", (long long)n);
         return GSB_ERR_OVERFLOW;
     }
     if (V > GSB_SORT_MAX_VIEWS) { set_error("sort_pairs: more than %d views", GSB_SORT_MAX_VIEWS); return GSB_ERR_ARGUMENT; }
-    return onesweep_sort(keys, vals, keys_alt, vals_alt, n, n_dev, begin_bit, end_bit, scratch, debug, stream, V, sv);
+    return onesweep_sort(keys, vals, keys_alt, vals_alt, n, n_dev, begin_bit, end_bit, scratch, debug, stream, V, sv, hist_ready);
 }
 
 }  // namespace gsb
