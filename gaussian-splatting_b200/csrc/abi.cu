@@ -635,6 +635,40 @@ int32_t gsb_render_features(int32_t V, const GsbState *states, int32_t height, i
     return launch_render_features(a, false, static_cast<cudaStream_t>(cuda_stream));
 }
 
+int32_t gsb_contribution(int32_t V, const GsbState *states, int32_t height, int32_t width, int32_t P, int64_t *count,
+                         float *weight_sum, float *weight_max, void *cuda_stream) {
+    if (!states || V < 1 || V > GSB_MAX_VIEWS || height <= 0 || width <= 0 || P < 0 ||
+        (P > 0 && (!count || !weight_sum || !weight_max))) {
+        set_error("gsb_contribution: NULL argument, V=%d outside 1..%d, bad image size %d x %d or P=%d", V, GSB_MAX_VIEWS, height,
+                  width, P);
+        return GSB_ERR_ARGUMENT;
+    }
+    if ((reinterpret_cast<size_t>(count) & 7) || misaligned(weight_sum) || misaligned(weight_max)) {
+        set_error("gsb_contribution: count must be 8-byte, weight_sum and weight_max 4-byte aligned");
+        return GSB_ERR_ARGUMENT;
+    }
+    ContribArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = width; a.H = height; a.gx = (width + TILE - 1) / TILE; a.gy = (height + TILE - 1) / TILE; a.V = V; a.P = P;
+    a.count = reinterpret_cast<long long *>(count); a.weight_sum = weight_sum;
+    a.weight_max_bits = reinterpret_cast<uint32_t *>(weight_max);
+    const size_t npix = (size_t)height * width;
+    for (int v = 0; v < V; ++v) {
+        if (states[v].P != P) {
+            set_error("gsb_contribution: state %d holds %d gaussians, not %d", v, states[v].P, P);
+            return GSB_ERR_ARGUMENT;
+        }
+        if (P == 0) continue;
+        // the IMAGE buffer holds final_T and n_contrib of npix pixels each (carve_image): a smaller one is another image size
+        if (!feat_view(states[v], P, a.gx * a.gy, a.view[v]) || !states[v].image ||
+            (const char *)states[v].n_contrib + npix * sizeof(uint32_t) > (const char *)states[v].image + states[v].image_bytes) {
+            set_error("gsb_contribution: state %d is not a forward of %d gaussians over %d x %d pixels", v, P, width, height);
+            return GSB_ERR_ARGUMENT;
+        }
+    }
+    return launch_contribution(a, false, static_cast<cudaStream_t>(cuda_stream));
+}
+
 static int check_batch(int32_t V, const GsbSettings *s, const GsbInputs *in, CamArgsBatch &cb) {
     if (V < 1 || V > GSB_MAX_VIEWS) { set_error("view batch: V=%d outside 1..%d", V, GSB_MAX_VIEWS); return GSB_ERR_ARGUMENT; }
     cb.V = V;
@@ -1233,6 +1267,36 @@ int32_t gsb_densify_apply(const GsbDensifyArgs *a, const float *unit_samples, in
     if (a->P == 0) return GSB_OK;
     return launch_densify_apply(a->P, a->sh_coeffs, a->n_children, a->params, a->exp_avg, a->exp_avg_sq, a->scratch, unit_samples,
                                 n_split, P_new, new_params, new_exp_avg, new_exp_avg_sq, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int32_t gsb_prune_plan(int64_t P, const uint8_t *remove, void *scratch, int64_t *P_new, void *cuda_stream) {
+    if (P < 0 || !P_new || !store_fits_u32(P, 1, 1) || (P > 0 && (!remove || !scratch))) {
+        set_error("gsb_prune_plan: bad argument");
+        return GSB_ERR_ARGUMENT;
+    }
+    *P_new = 0;
+    if (P == 0) return GSB_OK;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    uint32_t *dev = nullptr;
+    const int e = launch_prune_plan(P, remove, scratch, &dev, stream);
+    if (e) return e;
+    uint32_t host = 0;
+    GSB_CUDA(cudaMemcpyAsync(&host, dev, sizeof(host), cudaMemcpyDeviceToHost, stream));
+    GSB_CUDA(cudaStreamSynchronize(stream));
+    *P_new = host;
+    return GSB_OK;
+}
+
+int32_t gsb_prune_apply(int64_t P, int32_t sh_coeffs, const float *params, const float *exp_avg, const float *exp_avg_sq,
+                        const void *scratch, int64_t P_new, float *new_params, float *new_exp_avg, float *new_exp_avg_sq,
+                        void *cuda_stream) {
+    if (P < 0 || sh_coeffs < 1 || P_new < 0 || P_new > P || !store_fits_u32(P, sh_coeffs, 1) ||
+        (P_new > 0 && (!params || !exp_avg || !exp_avg_sq || !scratch || !new_params || !new_exp_avg || !new_exp_avg_sq))) {
+        set_error("gsb_prune_apply: bad argument");
+        return GSB_ERR_ARGUMENT;
+    }
+    return launch_prune_apply(P, sh_coeffs, params, exp_avg, exp_avg_sq, scratch, P_new, new_params, new_exp_avg, new_exp_avg_sq,
+                              static_cast<cudaStream_t>(cuda_stream));
 }
 
 int32_t gsb_knn_mean_dist2(const float *points, int64_t P, float *out, gsb_alloc_fn alloc, void *alloc_ctx, void *cuda_stream) {

@@ -282,4 +282,38 @@ int launch_densify_apply(int64_t P, int sh_coeffs, int n_children, const float *
     return GSB_OK;
 }
 
+// ---- prune_points (scene/gaussian_model.py:349-364): the densify pipeline with originals only --------------------------------
+// keep flags -> exclusive scan (output positions, P_new) -> source row of every output row -> densify_gather_kernel with
+// n_children = 1 and no clone / child slot kept, i.e. every output row an original that keeps its moments.
+__global__ void __launch_bounds__(DS_THREADS)
+prune_keep_kernel(const uint8_t *__restrict__ remove, const uint32_t P, uint32_t *__restrict__ keep) {
+    const uint32_t i = blockIdx.x * DS_THREADS + threadIdx.x;
+    if (i < P) keep[i] = remove[i] ? 0u : 1u;
+}
+
+int launch_prune_plan(int64_t P, const uint8_t *remove, void *scratch, uint32_t **counter_dev, cudaStream_t stream) {
+    const DensifyScratch s = carve_densify(scratch, P, 1, nullptr);
+    GSB_LAUNCH("prune_keep", false, stream, prune_keep_kernel, (uint32_t)ceil_div(P, DS_THREADS), DS_THREADS, 0, remove, (uint32_t)P, s.pos);
+    const int e = exclusive_scan_u32(s.pos, s.pos, (size_t)P, s.partials, s.counters + 3, stream);
+    if (e) return e;
+    GSB_LAUNCH("densify_invert", false, stream, densify_invert_kernel, (uint32_t)ceil_div(P, DS_THREADS), DS_THREADS, 0, s.pos,
+               s.counters + 3, (size_t)P, s.src);
+    *counter_dev = s.counters + 3;
+    return GSB_OK;
+}
+
+int launch_prune_apply(int64_t P, int sh_coeffs, const float *params, const float *m, const float *v, const void *scratch, int64_t P_new,
+                       float *new_params, float *new_m, float *new_v, cudaStream_t stream) {
+    if (P_new == 0) return GSB_OK;
+    const DensifyScratch s = carve_densify(const_cast<void *>(scratch), P, 1, nullptr);
+    GatherArgs a;
+    a.o = StoreLayout{(uint32_t)P, 3u * (uint32_t)sh_coeffs};
+    a.n = StoreLayout{(uint32_t)P_new, 3u * (uint32_t)sh_coeffs};
+    a.N = 1; a.n_split = 0u;
+    a.p = params; a.m = m; a.v = v; a.np = new_params; a.nm = new_m; a.nv = new_v;
+    a.src = s.src; a.rank = s.rank; a.unit = nullptr;
+    GSB_LAUNCH("densify_gather", false, stream, densify_gather_kernel, (uint32_t)ceil_div((int64_t)a.n.total(), DS_THREADS), DS_THREADS, 0, a);
+    return GSB_OK;
+}
+
 }  // namespace gsb

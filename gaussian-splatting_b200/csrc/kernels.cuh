@@ -152,6 +152,16 @@ struct FeatArgs {
     float *dL_dfeatures;                    // backward: [P, C], added into; NULL = not requested
 };
 
+// Contribution statistics (contrib.cu, DESIGN.md section 7.8): for every pair a forward state accepted, count[id] += 1,
+// weight_sum[id] += w and weight_max[id] = max(., w) with w = alpha T, over V <= GSB_MAX_VIEWS states (blockIdx.y = view).
+struct ContribArgs {
+    int W, H, gx, gy, V, P;
+    FeatView view[GSB_MAX_VIEWS];
+    long long *count;              // [P], added into
+    float *weight_sum;             // [P], added into
+    uint32_t *weight_max_bits;     // [P] float bits (w >= 0), max-ed into
+};
+
 // split: a.shs / a.rest are the split SH input (see PreFwdArgs)
 int launch_preprocess_fwd(const CamArgs &ca, const PreFwdArgs &a, bool split, bool debug, cudaStream_t stream);
 int launch_preprocess_bwd(const CamArgs &ca, const PreBwdArgs &a, bool split, bool accumulate, bool debug, cudaStream_t stream);
@@ -177,6 +187,7 @@ int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream);
 int launch_alpha(const AlphaArgs &a, bool debug, cudaStream_t stream);
 int launch_render_features(const FeatArgs &a, bool debug, cudaStream_t stream);
 int launch_render_features_bwd(const FeatArgs &a, bool debug, cudaStream_t stream);
+int launch_contribution(const ContribArgs &a, bool debug, cudaStream_t stream);
 int launch_tile_order(const uint2 *ranges, int V, int num_tiles, uint32_t *order, bool debug, cudaStream_t stream);
 int launch_l1_loss_grad(const float *img, const float *gt, int64_t n, float scale, float *grad, float *loss_accum,
                         cudaStream_t stream);
@@ -204,5 +215,10 @@ int launch_densify_plan(int64_t P, int sh_coeffs, int n_children, const float *p
 int launch_densify_apply(int64_t P, int sh_coeffs, int n_children, const float *params, const float *m, const float *v, void *scratch,
                          const float *unit_samples, int64_t n_split, int64_t P_new, float *new_params, float *new_m, float *new_v,
                          cudaStream_t stream);
+// prune_points on the store: scratch of densify_scratch_bytes(P, 1); plan = keep flags, their exclusive scan and the source row
+// of every output row (*counter_dev: the device word holding P_new), apply = the densify gather of the kept rows
+int launch_prune_plan(int64_t P, const uint8_t *remove, void *scratch, uint32_t **counter_dev, cudaStream_t stream);
+int launch_prune_apply(int64_t P, int sh_coeffs, const float *params, const float *m, const float *v, const void *scratch, int64_t P_new,
+                       float *new_params, float *new_m, float *new_v, cudaStream_t stream);
 
 }  // namespace gsb

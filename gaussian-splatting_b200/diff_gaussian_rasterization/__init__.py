@@ -25,7 +25,7 @@ from typing import NamedTuple, Optional
 import torch
 import torch.nn as nn
 
-__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians"]
+__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "ContributionStats"]
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 # GSB_LIBRARY: an alternative build of the same sources (A/B of compile-time knobs); default = the in-tree library
@@ -148,6 +148,8 @@ def _load(path: Optional[str] = None):
                                              c_void_p]
     lib.gsb_render_features.restype = c_int32
     lib.gsb_render_features.argtypes = [c_int32, POINTER(_State), c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.gsb_contribution.restype = c_int32
+    lib.gsb_contribution.argtypes = [c_int32, POINTER(_State), c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.gsb_backward_features.restype = c_int32
     lib.gsb_backward_features.argtypes = [POINTER(_Settings), POINTER(_Inputs), POINTER(_SplitSH), POINTER(_State), c_void_p,
                                           c_void_p, c_void_p, c_void_p, c_void_p, POINTER(_Grads), POINTER(_CameraGrads),
@@ -212,6 +214,11 @@ def _load(path: Optional[str] = None):
     lib.gsb_densify_plan.argtypes = [POINTER(_DensifyArgs), POINTER(c_int64 * 4), c_void_p]
     lib.gsb_densify_apply.restype = c_int32
     lib.gsb_densify_apply.argtypes = [POINTER(_DensifyArgs), c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.gsb_prune_plan.restype = c_int32
+    lib.gsb_prune_plan.argtypes = [c_int64, c_void_p, c_void_p, POINTER(c_int64), c_void_p]
+    lib.gsb_prune_apply.restype = c_int32
+    lib.gsb_prune_apply.argtypes = [c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]
     lib.gsb_knn_mean_dist2.restype = c_int32
     lib.gsb_knn_mean_dist2.argtypes = [c_void_p, c_int64, c_void_p, _ALLOC_FN, c_void_p, c_void_p]
     if lib.gsb_abi_version() != ABI_VERSION:
@@ -433,6 +440,28 @@ def densify_apply(args, unit_samples: Optional[torch.Tensor], n_split: int, P_ne
                                     new_exp_avg_sq.data_ptr(), stream))
 
 
+def prune_plan(remove: torch.Tensor, P: int):
+    """gsb_prune_plan: ``remove`` bool / uint8 [P] (True = the row goes).  Returns (scratch, P_new); one stream synchronisation."""
+    stream = _stream_of(remove)
+    rm = remove.reshape(-1)
+    rm = (rm if rm.dtype == torch.uint8 else rm.to(torch.uint8)).contiguous()
+    scratch = torch.empty(max(int(_C.gsb_densify_scratch_bytes(int(P), 1)), 1), dtype=torch.uint8, device=remove.device)
+    P_new = c_int64(0)
+    with _device_ctx(remove.device):
+        _check(_C.gsb_prune_plan(int(P), rm.data_ptr() if P > 0 else None, scratch.data_ptr(), byref(P_new), stream))
+    return scratch, int(P_new.value)
+
+
+def prune_apply(scratch: torch.Tensor, P: int, sh_coeffs: int, params, exp_avg, exp_avg_sq, P_new: int, new_params, new_exp_avg,
+                new_exp_avg_sq) -> None:
+    """gsb_prune_apply: one gather of the rows gsb_prune_plan kept into the new store and both moments."""
+    stream = _stream_of(params)
+    with _device_ctx(params.device):
+        _check(_C.gsb_prune_apply(int(P), int(sh_coeffs), params.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+                                  scratch.data_ptr(), int(P_new), new_params.data_ptr(), new_exp_avg.data_ptr(),
+                                  new_exp_avg_sq.data_ptr(), stream))
+
+
 def knn_mean_dist2(points: torch.Tensor) -> torch.Tensor:
     """Mean squared distance of every point [P,3] to its three nearest other points (gsb_knn_mean_dist2; the replacement of
     simple_knn._C.distCUDA2, scene/gaussian_model.py:159)."""
@@ -646,6 +675,59 @@ def _features_impl(states, height: int, width: int, features: torch.Tensor, devi
                                     features.data_ptr() if P > 0 else None, out.data_ptr(), _current_stream(device))
     _check(rc)
     return out[0] if one else out
+
+
+class ContributionStats:
+    """Per-gaussian contribution statistics of forward passes (gsb_contribution; definition in include/gs_b200.h), accumulated
+    over every view and call they are handed to (``contrib=`` of rasterize_gaussians / GaussianRasterizer / render /
+    render_views_backward):
+
+    * ``count`` int64 [P]: the number of (pixel, gaussian) pairs the forward blended;
+    * ``weight_sum`` float32 [P]: the sum of their blend weights alpha * T;
+    * ``weight_max`` float32 [P]: the largest of those weights, 0 for a gaussian that was never blended.
+
+    The usage scores of contribution-based pruning (sum of weights, max weight, pixel count).  Starts at zero; ``zero_()``
+    starts over.  A ``prune_points`` makes the statistics stale: take a new object for the new gaussians."""
+
+    def __init__(self, P: int, device):
+        self.P = int(P)
+        self.device = torch.device(device)
+        self.count = torch.zeros(self.P, dtype=torch.int64, device=self.device)
+        self.weight_sum = torch.zeros(self.P, dtype=torch.float32, device=self.device)
+        self.weight_max = torch.zeros(self.P, dtype=torch.float32, device=self.device)
+
+    def zero_(self):
+        self.count.zero_()
+        self.weight_sum.zero_()
+        self.weight_max.zero_()
+        return self
+
+
+def check_contrib(contrib, P: int, device) -> None:
+    """Raises ValueError unless ``contrib`` is a ContributionStats of P gaussians on ``device`` with intact tensors."""
+    if not isinstance(contrib, ContributionStats):
+        raise ValueError(f"contrib must be a ContributionStats; got {type(contrib).__name__}")
+    want = {"count": torch.int64, "weight_sum": torch.float32, "weight_max": torch.float32}
+    for name, dtype in want.items():
+        t = getattr(contrib, name)
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.dim() != 1 or not t.is_contiguous():
+            raise ValueError(f"contrib.{name} must be a contiguous 1-D {dtype} tensor")
+        if int(t.shape[0]) != int(P):
+            raise ValueError(f"contrib.{name} has {int(t.shape[0])} entries, the gaussians number {int(P)}")
+        if t.device != torch.device(device):
+            raise ValueError(f"contrib.{name} lives on {t.device}, the gaussians on {device}")
+
+
+def _contrib_impl(states, height: int, width: int, P: int, contrib: ContributionStats, device) -> None:
+    """Adds the contribution statistics of the forward states ``states`` (a ``_State`` or a ctypes array of them) into
+    ``contrib``.  One launch (none for P == 0), no synchronisation."""
+    one = isinstance(states, _State)
+    V = 1 if one else len(states)
+    with _device_ctx(device):
+        rc = _C.gsb_contribution(V, byref(states) if one else states, int(height), int(width), int(P),
+                                 contrib.count.data_ptr(), contrib.weight_sum.data_ptr(), contrib.weight_max.data_ptr(),
+                                 _current_stream(device))
+    _check(rc)
 
 
 def _feature_term(feats: Optional[dict]):
@@ -882,7 +964,7 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, dc=None, return_alpha=False, features=None):
+                        raster_settings, dc=None, return_alpha=False, features=None, contrib=None):
     """``dc`` (optional): split SH input -- ``dc`` [P,1,3] holds the DC coefficient and ``sh`` [P,M-1,3] the others (M-1 may
     be 0); the result equals that of ``sh = cat((dc, sh), 1)`` without the concatenation.
 
@@ -897,11 +979,17 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
     ``features`` [P, C] (1 <= C <= MAX_FEATURE_CHANNELS, view-independent): one more trailing output, the feature map [C,H,W]
     = sum_k alpha_k T_k features[k] with the forward's blend weights and background 0 (gsb_render_features; definition in
     include/gs_b200.h).  Its gradient reaches ``features`` and every gaussian and camera input.  One extra launch in the forward,
-    one in a backward that uses the map's gradient; without ``features`` the call is unchanged.  Bad shapes raise ValueError."""
+    one in a backward that uses the map's gradient; without ``features`` the call is unchanged.  Bad shapes raise ValueError.
+
+    ``contrib`` (a ContributionStats of P gaussians on the gaussians' device): the forward's per-gaussian contribution
+    statistics are added into it (gsb_contribution; one extra launch in the forward, outputs and gradients unchanged; also under
+    torch.no_grad()).  A wrong P, device or dtype raises ValueError."""
     if features is not None:
         check_features(features, int(means3D.shape[0]), means3D.device)
+    if contrib is not None:
+        check_contrib(contrib, int(means3D.shape[0]), means3D.device)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings, dc, bool(return_alpha), features,
+                                     cov3Ds_precomp, raster_settings, dc, bool(return_alpha), features, contrib,
                                      *_camera_inputs(raster_settings))
 
 
@@ -916,7 +1004,7 @@ def _camera_inputs(rs) -> tuple:
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, dc=None, return_alpha=False, features=None, *camera):
+                raster_settings, dc=None, return_alpha=False, features=None, contrib=None, *camera):
         # camera: the settings' (viewmatrix, projmatrix, campos, bg) as inputs of their own (rasterize_gaussians), or ()
         args = [_f32c(means3D), _f32c(sh), _f32c(colors_precomp), _f32c(opacities), _f32c(scales), _f32c(rotations),
                 _f32c(cov3Ds_precomp)]
@@ -943,6 +1031,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         if features is not None:
             fc = features.detach().float().contiguous()
             fmap = _features_impl(pack["state"], H, W, fc, color.device)
+        if contrib is not None:
+            _contrib_impl(pack["state"], H, W, int(args[0].shape[0]), contrib, color.device)
         ctx.save_for_backward(*[a if a is not None else torch.empty(0) for a in args], color, invdepth,
                               dcc if dcc is not None else torch.empty(0), *((fc, fmap) if fc is not None else ()))
         ctx.mark_non_differentiable(radii)
@@ -986,9 +1076,9 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads["scales"] = new(P, 3)
             grads["rotations"] = new(P, 4)
         cam_grads = {k: torch.empty(_CAMERA_NUMEL[k], dtype=torch.float32, device=dev)
-                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[12 + j]}
+                     for j, k in enumerate(CAMERA_KEYS) if ctx.camera and ctx.needs_input_grad[13 + j]}
         if grad_out_color is None and grad_out_depth is None and grad_out_alpha is None and grad_out_feat is None:
-            return (None,) * (12 + len(ctx.camera))
+            return (None,) * (13 + len(ctx.camera))
         gc = _f32c(grad_out_color)
         if gc is None:
             gc = torch.zeros((3, int(rs.image_height), int(rs.image_width)), dtype=torch.float32, device=dev)
@@ -1021,7 +1111,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grads["means3D"], grads["means2D"] if ctx.shapes["means2D"] is not None else None, grads.get("shs"),
                 grads.get("colors_precomp"), g_op, grads.get("scales"), grads.get("rotations"),
                 grads.get("cov3D_precomp"), None, grads.get("dc"), None,
-                feats["dL_dfeatures"] if feats is not None else None) + g_cam
+                feats["dL_dfeatures"] if feats is not None else None, None) + g_cam
 
 
 class GaussianRasterizer(nn.Module):
@@ -1045,11 +1135,12 @@ class GaussianRasterizer(nn.Module):
             return present.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None, dc=None, return_alpha=False, features=None):
+                cov3D_precomp=None, dc=None, return_alpha=False, features=None, contrib=None):
         """``dc``: the split SH input of the accel branch (gaussian_renderer/__init__.py:90-100) -- ``dc`` [P,1,3] is the DC
         coefficient and ``shs`` [P,M-1,3] the others (may have zero coefficients); gradients come back in the same split.
         ``return_alpha=True``: also returns the rendered alpha [1,H,W] (rasterize_gaussians).  ``features`` [P,C]: also returns
-        the feature map [C,H,W], last (rasterize_gaussians)."""
+        the feature map [C,H,W], last (rasterize_gaussians).  ``contrib`` (ContributionStats): the forward's contribution
+        statistics are added into it (rasterize_gaussians)."""
         rs = self.raster_settings
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
@@ -1059,7 +1150,7 @@ class GaussianRasterizer(nn.Module):
         if dc is not None and colors_precomp is not None:
             raise Exception("dc is the SH DC coefficient: it goes with shs, not with precomputed colors!")
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   rs, dc, return_alpha, features)
+                                   rs, dc, return_alpha, features, contrib)
 
 
 # SparseGaussianAdam: bound here only on request (module docstring); sparse_adam.py is importable either way

@@ -48,13 +48,14 @@ def _eval_sh(deg, sh, dirs):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, separate_sh=False,
-           override_color=None, use_trained_exp=False, return_alpha=False, features=None):
+           override_color=None, use_trained_exp=False, return_alpha=False, features=None, contrib=None):
     """Same contract as the reference's render(): returns
     {"render", "viewspace_points", "visibility_filter", "radii", "depth"}.  ``return_alpha=True`` adds "alpha": the rendered
     accumulated opacity [1,H,W] (1 - final transmittance, differentiable; the exposure of ``use_trained_exp`` does not apply).
     ``features`` [P,C] (per-gaussian, view-independent, 1 <= C <= 128) adds "features": the feature map [C,H,W] composited
     with the same blend weights over a zero background, differentiable w.r.t. ``features`` and the gaussians (no exposure,
-    no clamp)."""
+    no clamp).  ``contrib`` (diff_gaussian_rasterization.ContributionStats of the P gaussians): the view's per-gaussian
+    contribution statistics (blended pixel count, sum and max of the blend weights) are added into it; the result is unchanged."""
     xyz = pc.get_xyz
     screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
     try:
@@ -94,7 +95,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     out = rasterizer(means3D=xyz, means2D=screenspace_points, shs=shs, colors_precomp=colors_precomp, opacities=pc.get_opacity,
                      scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, dc=dc, return_alpha=return_alpha,
-                     features=features)
+                     features=features, contrib=contrib)
     rendered_image, radii, depth_image = out[:3]
 
     if use_trained_exp:
@@ -194,7 +195,7 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
                           scaling_modifier: float = 1.0, densify_stats: Optional[dict] = None,
                           keep_images: bool = False, loss_returns_grad: bool = False, batched: bool = True,
                           overwrite: bool = False, capacity: Optional[AsyncCapacity] = None, grad_chunks: int = 1,
-                          on_grad_chunk=None, peers=None, with_alpha: bool = False, features=None) -> dict:
+                          on_grad_chunk=None, peers=None, with_alpha: bool = False, features=None, contrib=None) -> dict:
     """Fused view-batch training step: forward + loss + backward for every camera, with the per-gaussian
     gradients of ALL views summed in place.
 
@@ -235,6 +236,10 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     ``dL/d feature map | None`` (the fourth, alpha's, may be None).  dL/dfeatures, summed over the views, goes into ``features``
     like a gaussian input's gradient, and the map's gradient into the same backward call.  Not with ``grad_chunks`` > 1,
     ``on_grad_chunk`` or ``peers`` (ValueError).  ``keep_images=True`` also returns "features" (the maps).
+
+    ``contrib`` (diff_gaussian_rasterization.ContributionStats of the P gaussians): every view's per-gaussian contribution
+    statistics are added into it, one launch per forward call (view-batch chunk or single view).  It only reads the forward
+    states, so it works in every mode (batched or not, sync or async, chunked, peers) and changes no output or gradient.
     """
     takes_grad_out = False
     if loss_returns_grad:
@@ -248,6 +253,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
     inputs = dict(means3D=xyz, shs=shs, opacities=opacity, scales=scales, rotations=rotations)
     P = int(xyz.shape[0])
     dev = xyz.device
+    if contrib is not None:
+        _dgr.check_contrib(contrib, P, dev)
 
     def grad_target(t):
         if t.is_leaf and t.requires_grad and t.grad is not None and t.grad.is_contiguous():
@@ -331,6 +338,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
             num_rendered.extend(pack["num_rendered"])
             alpha = _dgr._alpha_impl(pack["states"], int(color.shape[-2]), int(color.shape[-1]), dev) if with_alpha else None
             fmap = _dgr._features_impl(pack["states"], int(color.shape[-2]), int(color.shape[-1]), fc, dev) if fc is not None else None
+            if contrib is not None:
+                _dgr._contrib_impl(pack["states"], int(color.shape[-2]), int(color.shape[-1]), P, contrib, dev)
             g_color = torch.empty_like(color)
             g_depth = g_alpha = g_feat = None
             for k in range(len(chunk)):
@@ -386,6 +395,8 @@ def render_views_backward(viewpoint_cameras: Sequence, pc, pipe, bg_color: torch
         num_rendered.append(pack["num_rendered"])
         alpha = _dgr._alpha_impl(pack["state"], int(color.shape[-2]), int(color.shape[-1]), dev) if with_alpha else None
         fmap = _dgr._features_impl(pack["state"], int(color.shape[-2]), int(color.shape[-1]), fc, dev) if fc is not None else None
+        if contrib is not None:
+            _dgr._contrib_impl(pack["state"], int(color.shape[-2]), int(color.shape[-1]), P, contrib, dev)
         akw = dict(alpha=alpha) if with_alpha else {}
         if fc is not None:
             akw["features"] = fmap

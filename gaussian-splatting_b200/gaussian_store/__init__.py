@@ -416,6 +416,48 @@ class GaussianModel:
         self._skip_next = set(GROUPS)          # every parameter was replaced: the pending optimizer_step() is a no-op (see there)
         return {"n_clone": n_clone, "n_split": n_split, "n_pruned": n_pruned, "P": P_new}
 
+    def prune_points(self, mask: torch.Tensor) -> int:
+        """``prune_points(mask)`` of the reference (gaussian_model.py:349-364): rows with ``mask`` True (bool [P]) are removed,
+        the survivors keep their order, their parameters and both Adam moments, and every group keeps its step count.  The
+        densification statistics (``xyz_gradient_accum``, ``denom``, ``max_radii2D``) are gathered the same way; exposures are
+        untouched.  As in the reference, where every parameter becomes a fresh nn.Parameter with ``grad None``, the pending
+        ``optimizer_step()`` skips every group.  A plan (one read-back, of the new count) plus ONE gather of the store and both
+        moments (gsb_prune_plan / gsb_prune_apply).  Returns the new number of gaussians.
+
+        A typical mask is a contribution score: e.g. ``stats.weight_max < tau`` for a ``ContributionStats`` accumulated over the
+        training views (INTEGRATION.md)."""
+        if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or tuple(mask.shape) != (self.P,):
+            raise ValueError(f"prune_points: mask must be a bool tensor of shape ({self.P},)")
+        dev = self.store.device
+        if mask.device != dev:
+            raise ValueError(f"prune_points: mask lives on {mask.device}, the store on {dev}")
+        P, M = self.P, self.sh_coeffs
+        scratch, P_new = _dgr.prune_plan(mask, P)
+        total = store_offsets(P_new, M)["total"]
+        new = [torch.empty(total, dtype=torch.float32, device=dev) for _ in range(3)]
+        _dgr.prune_apply(scratch, P, M, self.store, self.exp_avg, self.exp_avg_sq, P_new, *new)
+        # the per-gaussian statistics: survivor i goes to row (number of survivors before i), removed rows to a spare row P_new
+        keep = ~mask
+        dest = torch.where(keep, torch.cumsum(keep, 0) - 1, torch.full((), P_new, dtype=torch.int64, device=dev))
+
+        def gather(t):
+            if t is None:
+                return None
+            out = t.new_empty((P_new + 1,) + tuple(t.shape[1:]))
+            out.index_copy_(0, dest, t)
+            return out[:P_new]
+
+        self.xyz_gradient_accum, self.denom = gather(self.xyz_gradient_accum), gather(self.denom)
+        self.max_radii2D = gather(self.max_radii2D)
+        self.P = P_new
+        self.store, self.exp_avg, self.exp_avg_sq = new
+        self.grad = torch.zeros(total, dtype=torch.float32, device=dev)
+        self.act = torch.empty(8 * P_new, dtype=torch.float32, device=dev)
+        self._bind()
+        self._reactivate()
+        self._skip_next = set(GROUPS)          # every parameter was replaced: the pending optimizer_step() is a no-op (see there)
+        return P_new
+
     def reset_opacity(self):
         """raw opacity <- logit(min(sigmoid(raw), 0.01)); the group's Adam moments restart at zero (:258-261, :302-314)."""
         o = store_offsets(self.P, self.sh_coeffs)

@@ -304,6 +304,21 @@ int32_t gsb_backward_batch_alpha(int32_t V, const GsbSettings *settings, const G
 int32_t gsb_render_features(int32_t V, const GsbState *states, int32_t height, int32_t width, int32_t P, int32_t channels,
                             const float *features, float *out, void *cuda_stream);
 
+/* Per-gaussian contribution statistics, DESIGN.md section 7.8: the usage scores of contribution-based pruning.  A forward state
+ * accepts a pair (pixel p, gaussian k) exactly when gsb_render_features does (power <= 0, alpha >= 1/255, list position <=
+ * n_contrib[p]); its blend weight is w_k(p) = alpha_k T_k, bit-equal to the weight of the blend.  Over the pixels of the V states:
+ *     count[k]      (int64)   += number of accepted pairs
+ *     weight_sum[k] (float32) += sum of w_k(p)
+ *     weight_max[k] (float32)  = max(weight_max[k], max of w_k(p))
+ * The outputs are ADDED into (max: max-ed into) so that views and calls accumulate; the caller zeroes them (weight_max >= 0
+ * then, and stays 0 for a gaussian without an accepted pair).  count and weight_max are deterministic; weight_sum depends on
+ * the order of float atomics.  The gaussian that would take T below 1e-4 is not blended and not counted.
+ * states[v] of any forward call (single view, split SH, view batch, async view batch); P and height x width must be theirs.
+ * One launch (none when P == 0), no host synchronisation; the states' BINNING, GEOM and IMAGE buffers must still be alive.
+ * count 8-byte aligned, weight_sum / weight_max 4-byte aligned; they may be NULL only when P == 0. */
+int32_t gsb_contribution(int32_t V, const GsbState *states, int32_t height, int32_t width, int32_t P, int64_t *count,
+                         float *weight_sum, float *weight_max, void *cuda_stream);
+
 /* The feature term of a backward call.  NULL pointers: no feature loss (dL_dout_features) or no feature gradient
  * (dL_dfeatures).  A NULL features pointer together with a non-NULL output is an error (unless P == 0). */
 typedef struct GsbFeatures {
@@ -455,6 +470,16 @@ int32_t gsb_densify_plan(const GsbDensifyArgs *args, int64_t counts[4], void *cu
 /* unit_samples: [n_children * n_split, 3] standard normals (the draw of torch.normal at :409). */
 int32_t gsb_densify_apply(const GsbDensifyArgs *args, const float *unit_samples, int64_t n_split, int64_t P_new,
                           float *new_params, float *new_exp_avg, float *new_exp_avg_sq, void *cuda_stream);
+
+/* prune_points(mask) (scene/gaussian_model.py:349-364) on the store: rows with remove[i] != 0 go, the survivors keep their order
+ * and their Adam moments.  scratch: gsb_densify_scratch_bytes(P, 1) bytes, written by plan and read by apply.
+ * gsb_prune_plan: keep flags, their exclusive scan and the source row of every output row; *P_new = survivors.  Synchronises
+ *   the stream once (the caller sizes the new store with P_new).
+ * gsb_prune_apply: one gather of the kept rows into new_params / new_exp_avg / new_exp_avg_sq (store layout of P_new rows). */
+int32_t gsb_prune_plan(int64_t P, const uint8_t *remove, void *scratch, int64_t *P_new, void *cuda_stream);
+int32_t gsb_prune_apply(int64_t P, int32_t sh_coeffs, const float *params, const float *exp_avg, const float *exp_avg_sq,
+                        const void *scratch, int64_t P_new, float *new_params, float *new_exp_avg, float *new_exp_avg_sq,
+                        void *cuda_stream);
 
 /* Mean squared distance from every point to its three nearest other points: the replacement of
  * simple_knn._C.distCUDA2 (scene/gaussian_model.py:21,159 -- initial scales).  points [P,3], out [P]; exact (uniform grid
