@@ -11,6 +11,7 @@
 namespace gsb {
 
 static thread_local char g_err[512] = "";
+static thread_local int g_deterministic = 0;    // gsb_set_deterministic: per host thread, like the last error
 int64_t g_launch_count = 0;
 
 int g_time_kernels = 0;
@@ -187,6 +188,11 @@ extern "C" {
 
 const char *gsb_last_error(void) { return g_err; }
 int32_t gsb_abi_version(void) { return GSB_ABI_VERSION; }
+int32_t gsb_set_deterministic(int32_t on) {
+    const int32_t prev = g_deterministic;
+    g_deterministic = on != 0;
+    return prev;
+}
 int64_t gsb_launch_count(void) { return g_launch_count; }
 void gsb_reset_launch_count(void) { g_launch_count = 0; }
 
@@ -447,6 +453,20 @@ static bool feat_view(const GsbState &st, int P, int num_tiles, FeatView &v) {
     return true;
 }
 
+// deterministic backward, first half: the partial rows and marks of the blend launch `ra` over V views of cap list positions
+// (GSB_BUF_SCRATCH2); launch_det_reduce after the blend launch stores the accumulator rows
+static int det_begin(const char *fn, gsb_alloc_fn alloc, void *alloc_ctx, int64_t cap, int V, DetScratch &d, RenderBwdArgs &ra,
+                     cudaStream_t stream) {
+    if (cap >= ((int64_t)1 << 30)) { set_error("%s: deterministic backward: capacity %lld exceeds 2^30", fn, (long long)cap); return GSB_ERR_OVERFLOW; }
+    const int64_t capn = cap > 0 ? cap : 1;
+    void *scr = do_alloc(alloc, alloc_ctx, GSB_BUF_SCRATCH2, det_carve(nullptr, capn, V, d));
+    if (!scr) return GSB_ERR_ALLOC;
+    det_carve(scr, capn, V, d);
+    GSB_CUDA(cudaMemsetAsync(d.mark, 0, (size_t)V * capn * 2, stream));
+    ra.det_part = d.part; ra.det_mark = d.mark;
+    return GSB_OK;
+}
+
 // shared body of gsb_backward (split == NULL), gsb_backward_split_sh, gsb_backward_camera (cam_grads != NULL),
 // gsb_backward_alpha (dL_dalpha != NULL) and gsb_backward_features (feat != NULL)
 static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *in, const GsbSplitSH *split, const GsbState *st,
@@ -480,6 +500,11 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
     bool want_feat = false;
     rc = check_features(fn, feat, P, want_feat);
     if (rc) return rc;
+    const bool det = g_deterministic != 0;
+    if (det && want_feat) {
+        set_error("%s: the feature backward has no deterministic implementation (gsb_set_deterministic is on)", fn);
+        return GSB_ERR_ARGUMENT;
+    }
     if (feat && feat->dL_dfeatures && !accumulate && P > 0)
         GSB_CUDA(cudaMemsetAsync(feat->dL_dfeatures, 0, (size_t)P * feat->channels * sizeof(float), stream));
     CamReduceArgs cr;
@@ -493,7 +518,7 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
     const size_t dacc_bytes = align_up((size_t)P * DACC_STRIDE * sizeof(float), 256);
     float *dacc = static_cast<float *>(do_alloc(alloc, alloc_ctx, GSB_BUF_SCRATCH0, dacc_bytes));
     if (!dacc) return GSB_ERR_ALLOC;
-    GSB_CUDA(cudaMemsetAsync(dacc, 0, dacc_bytes, stream));
+    if (!det || st->num_rendered == 0) GSB_CUDA(cudaMemsetAsync(dacc, 0, dacc_bytes, stream));     // det: det_reduce stores every row
     const float4 *splat = static_cast<const float4 *>(st->splat);
 
     if (st->num_rendered != 0) {
@@ -505,8 +530,11 @@ static int backward_impl(const char *fn, const GsbSettings *s, const GsbInputs *
         ra.splat = splat; ra.n_contrib = st->n_contrib; ra.dL_dcolor = dL_dcolor;
         ra.dL_dinvdepth = dL_dinvdepth; ra.dacc = dacc; ra.out_color = out_color; ra.out_invdepth = out_invdepth;
         ra.final_T = st->final_T; ra.dL_dalpha = dL_dalpha;
+        DetScratch ds;
+        if (det && (rc = det_begin(fn, alloc, alloc_ctx, st->binning_capacity, 1, ds, ra, stream))) return rc;
         rc = launch_render_bwd(ra, debug, stream);
         if (rc) return rc;
+        if (det && (rc = launch_det_reduce(ra, ds, P, dacc, debug, stream))) return rc;
         if (want_feat) {     // adds its terms into the same accumulator rows (linear in the loss gradient)
             FeatArgs fa;
             memset(&fa, 0, sizeof(fa));
@@ -902,6 +930,12 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
         set_error("gsb_backward_batch_features: features are not available on the chunked or peer backward");
         return GSB_ERR_ARGUMENT;
     }
+    const bool det = g_deterministic != 0;
+    if (det && (want_feat || peers)) {
+        set_error("gsb_backward_batch: the %s has no deterministic implementation (gsb_set_deterministic is on)",
+                  want_feat ? "feature backward" : "peer reduce-scatter");
+        return GSB_ERR_ARGUMENT;
+    }
     const bool debug = s[0].debug != 0;
     const CamArgs &c0 = cb.cam[0];
     const int P = in->P;
@@ -922,7 +956,7 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
     const size_t dacc_bytes = align_up((size_t)V * sv_dacc * sizeof(float), 256);
     float *dacc = static_cast<float *>(do_alloc(alloc, alloc_ctx, GSB_BUF_SCRATCH0, dacc_bytes));
     if (!dacc) return GSB_ERR_ALLOC;
-    GSB_CUDA(cudaMemsetAsync(dacc, 0, dacc_bytes, stream));
+    if (!det || !any) GSB_CUDA(cudaMemsetAsync(dacc, 0, dacc_bytes, stream));     // det: det_reduce stores every row
     if (feat && feat->dL_dfeatures && !accumulate)
         GSB_CUDA(cudaMemsetAsync(feat->dL_dfeatures, 0, (size_t)P * feat->channels * sizeof(float), stream));
     const size_t sv_splat = V > 1 ? (size_t)((const float4 *)states[1].splat - (const float4 *)states[0].splat) : 0;
@@ -941,8 +975,11 @@ static int backward_batch_impl(int32_t V, const GsbSettings *s, const GsbInputs 
         ra.splat = static_cast<const float4 *>(states[0].splat); ra.n_contrib = states[0].n_contrib;
         ra.dL_dcolor = dL_dcolor; ra.dL_dinvdepth = dL_dinvdepth; ra.dacc = dacc; ra.out_color = out_color; ra.out_invdepth = out_invdepth;
         ra.final_T = states[0].final_T; ra.dL_dalpha = dL_dalpha;     // final_T and n_contrib share the IMAGE stride sv_image
+        DetScratch ds;
+        if (det && (rc = det_begin("gsb_backward_batch", alloc, alloc_ctx, states[0].binning_capacity, V, ds, ra, stream))) return rc;
         rc = launch_render_bwd(ra, debug, stream);
         if (rc) return rc;
+        if (det && (rc = launch_det_reduce(ra, ds, P, dacc, debug, stream))) return rc;
         if (want_feat) {     // adds into the same accumulator rows, view v at rows v * P + id
             FeatArgs fa;
             memset(&fa, 0, sizeof(fa));

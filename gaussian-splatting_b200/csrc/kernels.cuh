@@ -121,6 +121,10 @@ struct RenderBwdArgs {
     // rendered-alpha gradient (alpha = 1 - final_T): dL_dalpha [V][H*W] at stride sv_depth, final_T at stride sv_image; NULL =
     // no alpha term.  Appended last so that the parameter offsets of the kernels that do not read them stay where they were.
     const float *final_T, *dL_dalpha;
+    // deterministic backward (DESIGN.md section 7.9), NULL = the plain kernel: det_part [V][sv_list * 2][DACC_STRIDE] partial rows,
+    // det_mark [V][sv_list * 2] bytes, zeroed by the caller; appended last, as above
+    float *det_part;
+    uint8_t *det_mark;
 };
 
 // alpha[v][p] = 1 - final_T[v][p] for V <= GSB_MAX_VIEWS forward states (any mix of single-view and view-batch calls)
@@ -185,6 +189,18 @@ int launch_tile_ranges(const uint32_t *sorted_tiles, int64_t D, const unsigned l
 int launch_render_fwd(const RenderFwdArgs &a, bool debug, cudaStream_t stream);
 int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream);
 int launch_alpha(const AlphaArgs &a, bool debug, cudaStream_t stream);
+// deterministic backward (deterministic.cu, DESIGN.md section 7.9): scratch of V views of capn list positions each
+struct DetScratch {
+    int64_t capn;
+    float *part;                      // [V][capn * 2][DACC_STRIDE] partial rows of render_bwd_kernel<..., DET>
+    uint8_t *mark;                    // [V][capn * 2] written-pair marks, zeroed before the blend launch
+    uint32_t *keys, *vals, *keys_alt, *vals_alt;   // [V][capn] (gaussian id, list position) pairs of the grouping sort
+    unsigned long long *count;        // [GSB_MAX_VIEWS] instances per view
+    char *sortscr;
+};
+size_t det_carve(void *base, int64_t capn, int V, DetScratch &d);    // base NULL: size only
+// after launch_render_bwd(a) with a.det_part / a.det_mark from d: every row view * P + g of dacc, g < P, is stored
+int launch_det_reduce(const RenderBwdArgs &a, const DetScratch &d, int P, float *dacc, bool debug, cudaStream_t stream);
 int launch_render_features(const FeatArgs &a, bool debug, cudaStream_t stream);
 int launch_render_features_bwd(const FeatArgs &a, bool debug, cudaStream_t stream);
 int launch_contribution(const ContribArgs &a, bool debug, cudaStream_t stream);

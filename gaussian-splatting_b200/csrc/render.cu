@@ -42,15 +42,16 @@ struct alignas(16) StagedRec {
     float4 q1;          // {B', opacity, r, g}
     float b, inv_z;
     uint32_t row;       // backward: row of the gradient accumulator (view * P + gaussian id)
-    uint32_t pad;
+    uint32_t pad;       // deterministic backward: the entry's position in the view's point list
 };
 static_assert(sizeof(StagedRec) == 48, "three 16-byte units");
 
-__device__ __forceinline__ void stage_record(StagedRec &dst, float4 q0, float4 q1, const float4 q2, const uint32_t row) {
+__device__ __forceinline__ void stage_record(StagedRec &dst, float4 q0, float4 q1, const float4 q2, const uint32_t row,
+                                             const uint32_t pad = 0u) {
     stage_scale(q0, q1);   // conic pre-scaled for the log2-domain exponent (blend_common.cuh): q0 = {x, y, A', C'}, q1 = {B', o, r, g}
     dst.w0 = make_ulonglong2(pk(q0.x, q0.y), pk(q0.z, q0.w));
     dst.q1 = q1;
-    dst.b = q2.x; dst.inv_z = q2.y; dst.row = row; dst.pad = 0u;
+    dst.b = q2.x; dst.inv_z = q2.y; dst.row = row; dst.pad = pad;
 }
 
 // per-view base pointers of a batched launch (blockIdx.y = view)
@@ -191,7 +192,10 @@ __device__ __forceinline__ void red_add_on(float *p, const bool on, const float 
 // ALPHA: the rendered alpha A = 1 - final_T is one more channel whose per-gaussian "colour" is 1 and whose background is 0:
 // g_k += dL/dA and S += dL/dA * A.  Then T_k - (A - F_k) / (1 - alpha_k) = T_final / (1 - alpha_k) = dA/dalpha_k, as it must.
 // It has no colour gradient, so the accumulator row and the reduction are those of the plain kernel.
-template <bool DEPTH, bool ALPHA, int MINB>
+// DET (deterministic backward, DESIGN.md section 7.9): the same sums are STORED, not added: warp w's sums for list position
+// pos go to partial row (pos * 2 + w) of the view, and the warp marks byte pos * 2 + w; det_reduce (deterministic.cu) adds
+// the marked partials of every gaussian in ascending list order.
+template <bool DEPTH, bool ALPHA, int MINB, bool DET = false>
 __global__ void __launch_bounds__(64, MINB)
 render_bwd_kernel(const RenderBwdArgs a) {
     constexpr int NT = 64;
@@ -258,7 +262,7 @@ render_bwd_kernel(const RenderBwdArgs a) {
             const float4 *rec = splat + (size_t)g * SPLAT_F4;
             const float4 q0 = __ldg(rec), q1 = __ldg(rec + 1), q2 = __ldg(rec + 2);
             smask[k] = (uint8_t)patch_mask(q0.x, q0.y, q0.z, q0.w, q1.x, q2.z, fox, foy);
-            stage_record(srec[k], q0, q1, q2, row0 + g);
+            stage_record(srec[k], q0, q1, q2, row0 + g, DET ? range.x + (uint32_t)(base + k) : 0u);
         }
         __syncthreads();
         // The loop's per-thread constants are formed here, once per round, from an opaque copy of the thread index: hoisted
@@ -271,7 +275,8 @@ render_bwd_kernel(const RenderBwdArgs a) {
 #endif
         const int lane = tr & 31;
         const int slot = (lane & 2) ? 4 + 5 * (lane >> 4) : ((lane >> 1) & 2) + ((lane >> 3) & 1) + 5 * (lane >> 4);
-        float *dacc_lane = a.dacc + slot;
+        // DET: the lane's address in the warp's partial row of list position 0 (the loop adds pos * 96 bytes)
+        float *dacc_lane = (DET ? a.det_part + (v * a.sv_list * 2 + (size_t)(tr >> 5)) * DACC_STRIDE : a.dacc) + slot;
         uint32_t lane_mask = 1u << lane;
 #ifndef GSB_HOST_EMUL
         asm volatile("" : "+l"(dacc_lane), "+r"(lane_mask));
@@ -335,7 +340,12 @@ render_bwd_kernel(const RenderBwdArgs a) {
             const LaneBits lb = lane_bits(lane_mask);
             float r = reduce10_transposed<DEPTH>(sum, lb);
             r = lb.b4 ? r : __fmul_rn(r, q1.y);          // lanes 0..15 hold sums 0..4: the moments' opacity factor
-            red_add_on(dacc_lane + (size_t)rec.row * DACC_STRIDE, (lane_mask & ADDS) != 0u, r);
+            if (DET) {
+                if (lane_mask & ADDS) dacc_lane[(size_t)rec.pad * (2 * DACC_STRIDE)] = r;
+                if (lane_mask & 1u) a.det_mark[(v * a.sv_list + rec.pad) * 2 + (size_t)(tr >> 5)] = 1u;
+            } else {
+                red_add_on(dacc_lane + (size_t)rec.row * DACC_STRIDE, (lane_mask & ADDS) != 0u, r);
+            }
         }
 #pragma unroll
         for (int i = 0; i < 4; ++i) rem[i] -= MP_R;
@@ -403,6 +413,23 @@ int launch_render_fwd(const RenderFwdArgs &a, bool debug, cudaStream_t stream) {
     return GSB_OK;
 }
 
+template <bool DET>
+static int launch_render_bwd_t(const RenderBwdArgs &a, const int tiles, bool debug, cudaStream_t stream) {
+    const char *name = DET ? "render_bwd_det" : "render_bwd";
+    if (a.dL_dalpha) {   // register budgets: DESIGN.md section 7.6
+        if (a.dL_dinvdepth) {
+            GSB_LAUNCH(name, debug, stream, (render_bwd_kernel<true, true, ALPHA_DEPTH_MINB, DET>), dim3(tiles, a.V), 64, 0, a);
+        } else {
+            GSB_LAUNCH(name, debug, stream, (render_bwd_kernel<false, true, ALPHA_MINB, DET>), dim3(tiles, a.V), 64, 0, a);
+        }
+    } else if (a.dL_dinvdepth) {
+        GSB_LAUNCH(name, debug, stream, (render_bwd_kernel<true, false, 12, DET>), dim3(tiles, a.V), 64, 0, a);
+    } else {   // register budget for 16 CTAs/SM (64 registers, no spills on sm_90a)
+        GSB_LAUNCH(name, debug, stream, (render_bwd_kernel<false, false, 16, DET>), dim3(tiles, a.V), 64, 0, a);
+    }
+    return GSB_OK;
+}
+
 int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream) {
     const int tiles = a.gx * a.gy;
     if (tiles <= 0) return GSB_OK;
@@ -412,18 +439,12 @@ int launch_render_bwd(const RenderBwdArgs &a, bool debug, cudaStream_t stream) {
         set_error("render_bwd: dL_dalpha without final_T");
         return GSB_ERR_ARGUMENT;
     }
-    if (a.dL_dalpha) {   // register budgets: DESIGN.md section 7.6
-        if (a.dL_dinvdepth) {
-            GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<true, true, ALPHA_DEPTH_MINB>), dim3(tiles, a.V), 64, 0, a);
-        } else {
-            GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<false, true, ALPHA_MINB>), dim3(tiles, a.V), 64, 0, a);
-        }
-    } else if (a.dL_dinvdepth) {
-        GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<true, false, 12>), dim3(tiles, a.V), 64, 0, a);
-    } else {   // register budget for 16 CTAs/SM (64 registers, no spills on sm_90a)
-        GSB_LAUNCH("render_bwd", debug, stream, (render_bwd_kernel<false, false, 16>), dim3(tiles, a.V), 64, 0, a);
+    if ((a.det_part == nullptr) != (a.det_mark == nullptr)) {
+        set_error("render_bwd: deterministic partials without marks");
+        return GSB_ERR_ARGUMENT;
     }
-    return GSB_OK;
+    if (a.det_part) return launch_render_bwd_t<true>(a, tiles, debug, stream);
+    return launch_render_bwd_t<false>(a, tiles, debug, stream);
 }
 
 // Rendered alpha of V forward states: one launch, blockIdx.y = view.  The forward leaves final_T in every state's IMAGE buffer;

@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import warnings
 from ctypes import CFUNCTYPE, POINTER, Structure, byref, c_char_p, c_float, c_int32, c_int64, c_size_t, c_void_p
 from typing import NamedTuple, Optional
 
@@ -204,6 +205,8 @@ def _load(path: Optional[str] = None):
     lib.gsb_kernel_time.argtypes = [c_char_p, POINTER(ctypes.c_double), POINTER(c_int64), c_int32]
     lib.gsb_set_option.restype = c_int32
     lib.gsb_set_option.argtypes = [c_char_p, c_int32]
+    lib.gsb_set_deterministic.restype = c_int32
+    lib.gsb_set_deterministic.argtypes = [c_int32]
     lib.gsb_adam_step.restype = c_int32
     lib.gsb_adam_step.argtypes = [POINTER(_AdamArgs), c_void_p]
     lib.gsb_activate.restype = c_int32
@@ -721,6 +724,7 @@ def check_contrib(contrib, P: int, device) -> None:
 def _contrib_impl(states, height: int, width: int, P: int, contrib: ContributionStats, device) -> None:
     """Adds the contribution statistics of the forward states ``states`` (a ``_State`` or a ctypes array of them) into
     ``contrib``.  One launch (none for P == 0), no synchronisation."""
+    _deterministic("contrib= (the float-atomic weight_sum of gsb_contribution)")
     one = isinstance(states, _State)
     V = 1 if one else len(states)
     with _device_ctx(device):
@@ -728,6 +732,23 @@ def _contrib_impl(states, height: int, width: int, P: int, contrib: Contribution
                                  contrib.count.data_ptr(), contrib.weight_sum.data_ptr(), contrib.weight_max.data_ptr(),
                                  _current_stream(device))
     _check(rc)
+
+
+def _deterministic(what: Optional[str] = None) -> bool:
+    """Whether the backward that follows must be deterministic: torch's ``use_deterministic_algorithms`` flag.  ``what`` names
+    a path with no deterministic implementation; under the flag it raises RuntimeError as torch's own such operations do, or
+    warns and takes the default path (returns False) with ``warn_only=True``."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return False
+    if what is None:
+        return True
+    msg = (f"{what} does not have a deterministic implementation, but you set 'torch.use_deterministic_algorithms(True)'. "
+           f"You can turn off determinism just for this operation, or you can use the 'warn_only=True' option, if that's "
+           f"acceptable for your application.")
+    if not torch.is_deterministic_algorithms_warn_only_enabled():
+        raise RuntimeError(msg)
+    warnings.warn(msg)
+    return False
 
 
 def _feature_term(feats: Optional[dict]):
@@ -797,6 +818,9 @@ def _backward_impl(pack, rs, means3D, sh, colors_precomp, opacities, scales, rot
         arena = _Arena(dev, stream)
         cg = _camera_grads(cam_grads)
         ft = _feature_term(feats)
+        det = _deterministic("the feature-map backward (features= with a loss on the map)"
+                             if ft is not None and ft.dL_dout_features and P > 0 else None)
+        _C.gsb_set_deterministic(int(det))
         if ft is not None:
             sp = _split_sh(dc, sh, grads) if dc is not None else None
             rc = _C.gsb_backward_features(byref(cs), byref(ci), byref(sp) if sp is not None else None, byref(pack["state"]),
@@ -915,6 +939,13 @@ def _backward_batch_impl(pack, settings_list, means3D, sh, opacities, scales, ro
             pt = _PeerTable()
             pt.world, pt.rank, pt.rows_per_rank, pt.reserved = int(world), int(rank), int(rows_per_rank), 0
             pt.base = (c_void_p * 16)(*([int(b) for b in bases] + [None] * (16 - len(bases))))
+        if ft is not None and ft.dL_dout_features:
+            det = _deterministic("the feature-map backward (features= with a loss on the map)")
+        elif pt is not None:
+            det = _deterministic("the peer gradient reduce-scatter (peers=)")
+        else:
+            det = _deterministic()
+        _C.gsb_set_deterministic(int(det))
         err = []
 
         def _cb(_ctx, chunk, p0, p1):

@@ -4,7 +4,8 @@
  * No torch types, no exceptions.  Process-wide state, all of it listed here: the tuning options
  * (gsb_set_option: set them before the first call and leave them alone while calls are in flight),
  * the launch counter and the kernel-timing records (diagnostics, mutex-guarded).  Per host thread:
- * the last error string and one pinned read-back slot + event per device.
+ * the last error string, the deterministic switch (gsb_set_deterministic) and one pinned read-back slot +
+ * event per device.
  * Threading: any number of host threads may call concurrently (different streams / devices); the
  * reference calls from its single training thread (train.py), one process per GPU.
  *
@@ -495,6 +496,19 @@ void gsb_reset_launch_count(void);
 /* CUDA-event time of the launches of kernel `name` ("" = all) recorded on their launching stream since
  * the last reset, while option "time_kernels" was 1 (blend kernels) or 2 (all).  Synchronises on the events. */
 int32_t gsb_kernel_time(const char *name, double *total_ms, int64_t *launches, int32_t reset);
+/* Deterministic backward switch of the CALLING HOST THREAD (off by default); returns the previous value.  Per thread
+ * because autograd runs CUDA backwards on its own device threads.  While it is on, every gradient output of every backward
+ * entry point (single view, split SH, camera, alpha; view batch plain, camera, chunked, after a sync or async forward) is a
+ * function of the forward state and the loss gradients alone: the blend kernel stores its per-(list entry, warp) sums
+ * instead of adding them with float atomics, and they are summed per gaussian in ascending list order.  Repeating a call
+ * gives identical bits whatever the CTA scheduling, the "tile_order" option or the chunking.  The values differ from the
+ * default path only by float reassociation.  Costs 4 + ceil(ceil(log2 P) / 8) kernel launches more per call and scratch
+ * (GSB_BUF_SCRATCH2) of about 114 bytes per instance of the forward's capacity, per view.
+ * No deterministic implementation, GSB_ERR_ARGUMENT while it is on: a feature term with a feature-map gradient
+ * (gsb_backward_features, gsb_backward_batch_features) and peers (gsb_backward_batch_peer, gsb_backward_batch_alpha /
+ * _features with a peer table).  Not covered (float atomics, whatever the switch): gsb_contribution's weight_sum and the
+ * loss scalars of gsb_l1_loss_grad / gsb_photometric_loss_grad (their gradients are per pixel and deterministic). */
+int32_t gsb_set_deterministic(int32_t on);
 /* tuning knobs (integers): "cull", "sort_small", "tile_order", "pre_tma", "time_kernels"; returns 0 if known */
 int32_t gsb_set_option(const char *name, int32_t value);
 
